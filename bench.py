@@ -48,7 +48,8 @@ import torch  # noqa: E402
 import torch.distributed as dist  # noqa: E402
 
 METRIC = "checkpoint_snapshot_GBps"
-HBM_FALLBACK_GBS = 6650.0  # /opt/skills/guides/B200_PROFILING.md fallback
+HBM_FALLBACK_GBS = 3350.0  # H100 SXM data sheet (HBM3); a copy peak measured on the box replaces it (MEASURED_PEAKS.json)
+DUMP_BYTES = 64 << 20  # --dump-outputs: upper bound of what is written
 WORKLOADS = {
     "c2": "C2: 16.06 GB Llama-3-8B-shaped param+Adam state_dict per rank (1164 fp32 tensors + 291 scalar steps), "
           "snapshot through TorchAsyncCheckpoint.async_save -> pinned host -> file on /dev/shm",
@@ -116,7 +117,7 @@ def flatten(sd):
 # helpers
 # ----------------------------------------------------------------------------------------------------
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled while the timed region runs (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled while the timed region runs."""
 
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -174,22 +175,7 @@ def hbm_peak():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:  # noqa: BLE001
             pass
-    return HBM_FALLBACK_GBS, "fallback (B200_PROFILING.md)"
-
-
-def ncu_traffic(label_prefix):
-    """dram read+write bytes per launch of the dominant kernel from the newest committed `ncu --set full` summary, with the
-    commit that summary was captured at (the number is a cross-check, not a live measurement)."""
-    for name in ("r02_ncu_walk_summary.json", "r01_ncu_walk_summary.json"):
-        p = ROOT / "profiles" / name
-        try:
-            doc = json.load(open(p))
-            for k in doc["kernels"]:
-                if k["label"].startswith(label_prefix):
-                    return float(k["traffic_bytes"]), f"profiles/{name} (ncu --set full, same state, one launch; captured at commit {doc.get('commit', 'round 1')})"
-        except Exception:  # noqa: BLE001
-            continue
-    return None, None
+    return HBM_FALLBACK_GBS, "H100 SXM data sheet (not measured)"
 
 
 def init_dist(n_gpus):
@@ -230,6 +216,40 @@ def shm_dir(rank, tag="bench"):
     d = base / f"nvrx_b200_{tag}_{os.getpid()}_{rank}"
     d.mkdir(parents=True, exist_ok=True)
     return d
+
+
+def dump_outputs(path, out_dir):
+    """What a caller of the timed path receives from its last step -- the state dict ``torch.load`` reads back from the
+    checkpoint file -- as ``out_dir/<key path>.npy``: float64 for 64-bit and integer tensors, float32 otherwise (bf16
+    widens exactly).  Tensors share DUMP_BYTES evenly; one larger than its share contributes a sample of its elements at
+    indices drawn from a seed derived from its key, the same on every run."""
+    import zlib
+
+    import numpy as np
+
+    named = []
+
+    def walk(x, prefix):
+        for k, v in (x.items() if isinstance(x, dict) else enumerate(x)):
+            key = f"{prefix}.{k}" if prefix else str(k)
+            if isinstance(v, (dict, list, tuple)):
+                walk(v, key)
+            elif isinstance(v, torch.Tensor):
+                named.append((key, v))
+
+    walk(torch.load(path, weights_only=False, mmap=True), "")
+    per_tensor = max(1, DUMP_BYTES // (8 * max(1, len(named))))
+    out_dir = Path(out_dir)
+    out_dir.mkdir(parents=True, exist_ok=True)
+    for key, t in named:
+        flat = t.detach().reshape(-1)
+        if flat.numel() > per_tensor:
+            rng = np.random.default_rng(zlib.crc32(key.encode()))
+            idx = np.sort(rng.integers(0, flat.numel(), size=per_tensor))
+            flat = flat[torch.from_numpy(idx)]
+        wide = t.dtype in (torch.float64, torch.int64, torch.int32, torch.uint8, torch.int8, torch.int16, torch.bool)
+        np.save(out_dir / f"{key.replace('/', '_')}.npy", flat.to(torch.float64 if wide else torch.float32).numpy())
+    return len(named)
 
 
 def bits_equal(a, b):
@@ -413,8 +433,7 @@ def d2h_ceiling(dev, world, gib=4, reps=4):
     """What the box gives N concurrent plain device->pinned-host copies (cudaMemcpyAsync into a cudaHostAlloc buffer, all
     ranks at once): the PCIe / host-memory ceiling the e2e number can be judged against.  The buffer is allocated while the
     thread is bound to the CPUs next to the GPU: where a pinned buffer lands is otherwise a lottery, and a buffer on the other
-    socket halves the rate when all 8 GPUs copy (16-21 instead of 39 GB/s per GPU on this pool's 8-GPU box,
-    profiles/r02_d2h_ceiling_8gpu.jsonl)."""
+    socket can halve the rate when all 8 GPUs copy."""
     n, rate, err, cpus, src, dst = gib << 30, None, None, None, None, None
     try:
         src = torch.empty(n, dtype=torch.uint8, device=dev)
@@ -616,6 +635,8 @@ def run_arm(args, rank, world, local):
             ok &= bits_equal(a, b.to(torch.bfloat16).cpu() if narrowed else b.cpu())
         check = "bit-exact" if ok else "MISMATCH"
         del loaded, lt
+    if rank == 0 and args.dump_outputs:
+        dump_outputs(path, args.dump_outputs)  # before the training-loop leg saves to the same path again
 
     load_ms = base_ms = None
     if not args.no_training_loop:
@@ -658,7 +679,7 @@ def run_arm(args, rank, world, local):
             "workload": WORKLOADS[args.config],
             "state_bytes_per_rank": total,
             "tensors": len(tensors),
-            "l2": "inputs (16 GB) >> L2 (126 MB); no flush needed",
+            "l2": "inputs (16 GB) >> L2 (50 MB); no flush needed",
             "scale": args.scale,
         },  # identical in both arms (the driver compares it); what differs between the arms is under "path" / "engine"
         "path": ("nvidia_resiliency_ext...TorchAsyncCheckpoint.async_save (pack kernel on the training stream, side-stream drain, "
@@ -695,7 +716,7 @@ def run_arm(args, rank, world, local):
         peak, peak_src = hbm_peak()
         algo = plan.algorithmic_bytes
         achieved = algo / (kernel_ms * 1e-3) / 1e9
-        traffic, traffic_src = (args.traffic_bytes, "command line") if args.traffic_bytes else ncu_traffic("pack LDG narrow" if args.narrow else "pack TMA")
+        traffic, traffic_src = (args.traffic_bytes, "command line") if args.traffic_bytes else (None, None)
         line["engine"] = {"packed_bytes_per_rank": plan.staging_bytes, "walker": os.environ.get("NVRX_B200_VARIANT", "auto")}
         line["roofline"] = {
             "bound": "hbm", "achieved": round(achieved, 1), "peak": peak, "unit": "GB/s", "frac": round(achieved / peak, 4),
@@ -767,7 +788,11 @@ def main():
     ap.add_argument("--no-ceiling", action="store_true")
     ap.add_argument("--no-c3-kernel", action="store_true", help="skip the C3 (narrowing) kernel-only leg of the default run")
     ap.add_argument("--traffic-bytes", type=float, default=None, help="dram read+write bytes per launch from the ncu capture")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what rank 0's last step saved (a fixed sample, <= 64 MB) as DIR/<key>.npy")
     args, rest = ap.parse_known_args()
+    if args.dump_outputs and args.config == "c4":
+        ap.error("--dump-outputs covers the c2 / c3 workloads")
     if args.narrow:
         args.config = "c3"
     args.narrow = args.config == "c3"

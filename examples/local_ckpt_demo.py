@@ -26,7 +26,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--ckpt_dir", default="/dev/shm/nvrx_b200_demo")
     ap.add_argument("--replication", action="store_true")
-    ap.add_argument("--sharded", action="store_true", help="striped fragments instead of full replicas (B200 extension)")
+    ap.add_argument("--sharded", action="store_true", help="striped fragments instead of full replicas (extension of this package)")
     args = ap.parse_args()
     rank, world, local = (int(os.environ.get(k, d)) for k, d in (("RANK", "0"), ("WORLD_SIZE", "1"), ("LOCAL_RANK", "0")))
     torch.cuda.set_device(local)

@@ -1,5 +1,5 @@
 /*
- * nvrx_snap.h -- C ABI of libnvrx_snap.so, the B200 (sm_100a) checkpoint-snapshot engine.
+ * nvrx_snap.h -- C ABI of libnvrx_snap.so, the H100 (sm_90a) checkpoint-snapshot engine.
  *
  * This is the drop-in boundary *below* the NVRx Python API.  The reference has no FFI for this path
  * (it is pure Python on top of PyTorch), so every entry point below names the reference code it

@@ -355,7 +355,7 @@ int nvrx_hostbuf_writev_fd(nvrx_hostbuf* hb, int64_t n, const uint64_t* offsets,
         // Allocate the destination range up front.  (1) A store into a mapping of a sparse file that the file system cannot
         // back (ENOSPC on the local SSD, tmpfs size limit, cgroup memory limit) is a SIGBUS that kills the writer with no
         // message; posix_fallocate reports the same condition as an errno.  (2) One in-kernel allocation pass is cheaper than
-        // one page fault per 4 KiB from 16 threads (16 GB into a fresh /dev/shm file: 4.9 s instead of 6.4 s on the B200 box).
+        // one page fault per 4 KiB from 16 threads (measurably faster for a fresh 16 GB /dev/shm file).
         const int rc = posix_fallocate(fd, static_cast<off_t>(map_lo), static_cast<off_t>(hi - map_lo));
         if (rc == EOPNOTSUPP || rc == EINVAL || rc == ENOSYS) {
             may_map = false;  // cannot pre-allocate here: use pwrite, whose errors are errnos as well

@@ -62,6 +62,13 @@ int ring_for(int device, uint64_t chunk, int slots, Ring** out) {
         const uint64_t bytes = chunk * static_cast<uint64_t>(slots);
         void* p = mmap(nullptr, bytes, PROT_READ | PROT_WRITE, MAP_PRIVATE | MAP_ANONYMOUS, -1, 0);
         if (p == MAP_FAILED) return NVRX_E_NOMEM;
+        // writer processes are forked later: a private mapping would turn copy-on-write at fork(), the readers' pread() would
+        // then land in fresh pages while the DMA mapping still points at the old ones (the H2D sends stale bytes).  No child
+        // uses the ring, so it is not inherited at all.
+        if (madvise(p, bytes, MADV_DONTFORK) != 0) {
+            munmap(p, bytes);
+            return NVRX_E_SYS;
+        }
         r.have_cpus = !getenv("NVRX_B200_NO_NUMA") && nvrx::numa_cpus_of_device(device, &r.cpus);
         {
             uint8_t* b = static_cast<uint8_t*>(p);

@@ -141,7 +141,7 @@ int build_tiles(nvrx_plan* p) {
             // this GPU are spread evenly over ALL destination GPUs (each peer gets 1/n of this GPU's NVLink egress, and
             // receives 1/n from each of its n senders) -- no destination sees more than one GPU's worth of ingress, whatever
             // the relative progress of the ranks.  Walking the shards one after the other made every rank store into the
-            // same one or two peers at a time (incast: 228 GB/s per GPU at 8 GPUs, profiles/r01_c4_kernel_only_8gpu.json).
+            // same one or two peers at a time (incast).
             auto weave = [&](std::vector<TileDesc>& v) {
                 if (v.empty()) return;
                 const uint64_t n_shards = (p->staging_bytes + p->shard_bytes - 1) / p->shard_bytes;
@@ -257,8 +257,8 @@ int upload(nvrx_plan* p, cudaStream_t st) {
 constexpr size_t kSmemBudget = 200 * 1024;
 
 int pick_stages(uint32_t tile_bytes) {
-    // measured on B200, 16 GB Llama-shaped state (profiles/r01_selftest_sweep.log): 32 KiB x 4 stages x 1 CTA/SM
-    // is the fastest ring (6.49 TB/s algorithmic); 16 KiB x 6 x 2 CTAs/SM and 64 KiB x 3 are within 2 %.
+    // default: 32 KiB x 4 stages x 1 CTA/SM (128 KiB of the 227 KiB an H100 block may have); tools/gpu_selftest.py sweeps
+    // the alternatives (16 KiB x 6 x 2 CTAs/SM, 64 KiB x 3) on the card at hand.
     static const int kChoices[] = {12, 8, 6, 4, 3};
     int want = tile_bytes >= 65536 ? 3 : tile_bytes >= 32768 ? 4 : tile_bytes >= 16384 ? 6 : 12;
     if (const char* env = getenv("NVRX_B200_TMA_STAGES")) want = atoi(env);
@@ -298,7 +298,7 @@ int launch_span(nvrx_plan* p, const TileSpan& span, uint8_t* staging, const Peer
             default: return launch_tma<DIR, 3, 2>(p, span, staging, pm, st);
         }
     }
-    uint32_t per_sm = 8;  // measured: 8 CTAs/SM worth of grid beats 4 (profiles/r01_selftest_sweep2.log)
+    uint32_t per_sm = 8;  // grid of 8 CTAs per SM (tools/gpu_selftest.py sweeps it)
     if (const char* env = getenv("NVRX_B200_LDG_CTAS_PER_SM")) per_sm = std::max(1, atoi(env));
     uint32_t grid = static_cast<uint32_t>(p->sm_count) * per_sm;
     grid = std::max<uint32_t>(1, std::min(grid, span.na + span.nb));

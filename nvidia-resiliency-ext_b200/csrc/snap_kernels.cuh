@@ -1,4 +1,4 @@
-// snap_kernels.cuh -- sm_100a device code of the snapshot engine: the tile walkers that pack a flattened
+// snap_kernels.cuh -- sm_90a device code of the snapshot engine: the tile walkers that pack a flattened
 // TensorAwareStateDict into one staging buffer and scatter it back.
 //
 // Pure data movement (no tensor cores): the roofline is HBM bandwidth, algorithmic traffic 2*S bytes per

@@ -73,13 +73,12 @@ class TorchAsyncCheckpoint(object):
             return 0
         from ..b200.engine import SnapshotEngine
         from ..b200.fastsave import zero_copy_enabled
-        from ..b200.ptzip import slot_tail_room
 
         engine = SnapshotEngine.get(cuda[0].device.index)
         cuda = [t if t.is_contiguous() else t.contiguous() for t in cuda]
         container = zero_copy_enabled() and len(cuda) == len(tensors)
         plan = engine._plan_for(cuda, engine._narrow_mask(cuda, self._narrow), container)
-        engine.reserve(plan.staging_bytes + (slot_tail_room(len(cuda)) if container else 0))
+        engine.reserve(plan.staging_bytes, len(cuda))
         return plan.staging_bytes
 
     def _reap(self, finalized=None):

@@ -196,7 +196,7 @@ def lib() -> C.CDLL:
                 E_STATE,
                 "loading libnvrx_snap.so",
                 f"{path} not found - run `python -c 'import __graft_entry__ as g; g.build()'` "
-                "(nvcc, sm_100a); there is no CPU fallback for the snapshot path",
+                "(nvcc, sm_90a); there is no CPU fallback for the snapshot path",
             )
         handle = C.CDLL(str(path), use_errno=True)
         _declare(handle)

@@ -1,4 +1,4 @@
-"""Host side of the B200 snapshot engine: thin objects over the C ABI plus the snapshot pipeline.
+"""Host side of the H100 snapshot engine: thin objects over the C ABI plus the snapshot pipeline.
 
 Pipeline of one snapshot (``SnapshotEngine.snapshot``)::
 
@@ -739,13 +739,19 @@ class SnapshotEngine:
         """Slots a snapshot could go to without giving up a published checkpoint: idle unpublished ones plus pool headroom."""
         return spare_slots(self._slots, self.max_host_slots)
 
-    def reserve(self, nbytes: int) -> None:
-        """Pre-allocate staging and every host slot for snapshots of up to ``nbytes`` packed bytes (pinning
-        16 GB takes seconds; do it once at start-up instead of inside the first save)."""
+    def reserve(self, nbytes: int, n_tensors: int = 0) -> None:
+        """Pre-allocate staging and every host slot for snapshots of up to ``nbytes`` packed bytes of ``n_tensors``
+        tensors (pinning 16 GB takes seconds; do it once at start-up instead of inside the first save).  With zero-copy
+        persistence on, a slot also holds the checkpoint file's small records and directory behind the payload: that
+        room is reserved too, or the first save would re-create and re-pin the slot."""
+        from .fastsave import zero_copy_enabled
+        from .ptzip import slot_tail_room
+
         self._ensure_staging(nbytes)
+        slot_bytes = nbytes + (slot_tail_room(n_tensors) if zero_copy_enabled() else 0)
         for s in self._slots:
             if not s.busy and not s.published():
-                self._acquire_slot(nbytes, s)
+                self._acquire_slot(slot_bytes, s)
                 self._release(s)
 
     # ---- planning -------------------------------------------------------------------------------

@@ -77,10 +77,10 @@ def _locate(ptr: int, nbytes: int):
 
 
 def zero_copy_enabled() -> bool:
-    """Default ON since round 2 (validated on B200: tests/test_gpu_zzero_copy.py): snapshots are packed in checkpoint-container
+    """Default ON (tests/test_gpu_zzero_copy.py): snapshots are packed in checkpoint-container
     geometry and a save whose target shares a file system with the slots (``/dev/shm``) publishes the slot with a hard link
-    instead of copying it -- writing 16 GB into a fresh tmpfs file is bounded by the kernel's page allocation at 2-4 GB/s
-    whatever the number of writers (profiles/r02_*), the link takes milliseconds.  Targets on other file systems, state dicts
+    instead of copying it -- writing 16 GB into a fresh tmpfs file is bounded by the kernel's page allocation whatever
+    the number of writers, the link takes milliseconds.  Targets on other file systems, state dicts
     with host tensors and saves that would take the last unpublished slot fall back to the copying writer by themselves.
     ``NVRX_B200_ZERO_COPY=0`` always copies (a published file shares its pages with the slot, see DESIGN.md for the caveat)."""
     return os.environ.get("NVRX_B200_ZERO_COPY", "1") != "0"

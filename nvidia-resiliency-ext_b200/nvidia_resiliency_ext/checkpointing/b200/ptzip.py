@@ -160,7 +160,7 @@ def small_records(obj: Any, protocol: int = torch.serialization.DEFAULT_PROTOCOL
 
     PyTorch itself produces them: ``torch.save`` with the data skipped into a scratch FILE, which the writer leaves sparse
     (it seeks over the records).  An in-memory ``BytesIO`` target must not be used here: seeking over 16 GB of skipped records
-    and then writing makes it allocate and zero all of it (8 s per checkpoint, measured on the B200 box in round 2)."""
+    and then writing makes it allocate and zero all of it (seconds per checkpoint)."""
     import tempfile
 
     scratch_dir = "/dev/shm" if os.access("/dev/shm", os.W_OK) else None
@@ -441,6 +441,8 @@ def tensor_offsets_in_file(path, tensors: Sequence[torch.Tensor]) -> Optional[Li
             if len(live) > 1 and all(reader.has_record(f"data/{i}") and reader.get_record_offset(f"data/{i}") == t.data_ptr() - guess for i, t in live):
                 base = guess
         if base is None:
+            if len(live) < 2:
+                return None  # one tensor fits under every record: only the maps entry can place it
             candidates = [first_t.data_ptr() - off0 for off0 in sorted(recs)]
             good = [g for g in candidates if g % 4096 == 0 and fits(g)]
             if len(good) != 1:

@@ -1,7 +1,7 @@
 """``ShardedLocalCheckpointManager``: local checkpoints whose replicas are *striped* over the clique (opt-in, new).
 
 The reference replicates by full copies (``CliqueReplicationStrategy``: every member stores every member's shard,
-``local/replication/strategies.py:88-140``).  This manager implements the layout of the B200 north star instead: the packed
+``local/replication/strategies.py:88-140``).  This manager implements the layout of the project's north star instead: the packed
 snapshot of rank *r* is cut into ``F-1`` equal fragments, fragment *k* goes to the *k*-th other member of *r*'s clique with
 ONE all-to-all over NVLink, and every rank stores
 
@@ -321,9 +321,8 @@ class ShardedLocalCheckpointManager(LocalCheckpointManager):
         for m, meta in zip(self._members, metas):
             lo, hi = (0, 0) if m == me else fragment_range(meta["total"], meta["shard_bytes"], self._others(m).index(me))
             recv_sizes.append(hi - lo)
-        # Round 1 (profiles/r01_c4_kernel_only_*gpu.json, 16 GB/rank): with 2 members the fused kernel beat pack + NCCL (23.3 vs
-        # 34.0 ms); with 8 members every rank walked its fragments in the same order, all senders hit the same destination at
-        # the same time (incast) and it lost (70.4 vs 29.9 ms).  Since round 2 the tile list of a sharded plan interleaves the
+        # If every rank walked its fragments in the same order, all senders would hit the same destination at the same time
+        # (incast).  The tile list of a sharded plan interleaves the
         # fragments (destination-major order, csrc/snap_api.cu build_tiles), every GPU stores to all peers at once, and the
         # fused kernel is the default whenever the clique is NVLink-peer reachable; NVRX_B200_EXCHANGE=nccl keeps pack + NCCL.
         if bases is not None:

@@ -1,7 +1,7 @@
 """Shared helpers of the checkpointing package.
 
 Mirror of the reference module ``checkpointing/utils.py`` (same public names) with ``preload_tensors``
-rebuilt on the B200 snapshot engine:
+rebuilt on the H100 snapshot engine:
 
 * ``preload_tensors``      reference ``utils.py:85-99``   -> one pack kernel + one side-stream drain
 * ``debug_time`` & friends reference ``utils.py:34-82``   -> same log format ("<stack> took X.XXXXs"), the

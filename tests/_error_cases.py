@@ -5,15 +5,16 @@ import os
 import re
 
 
-def _outcome(fn):
+def _outcome(fn, root):
     try:
         return {"returns": _plain(fn())}
     except BaseException as exc:  # noqa: BLE001 - the raised type is the point
-        return {"raises": type(exc).__name__, "message": _scrub(str(exc))}
+        return {"raises": type(exc).__name__, "message": _scrub(str(exc), root)}
 
 
-def _scrub(text):
-    text = re.sub(r"/tmp/[^\s'\"]+|/dev/shm/[^\s'\"]+", "<path>", text)
+def _scrub(text, root):
+    # the scenario root need not be under /tmp (TMPDIR, --basetemp): its paths are scrubbed wherever it is
+    text = re.sub(re.escape(root) + r"[^\s'\"]*|/tmp/[^\s'\"]+|/dev/shm/[^\s'\"]+", "<path>", text)
     return re.sub(r"0x[0-9a-f]+", "<addr>", text)
 
 
@@ -52,6 +53,9 @@ def scenarios(tmp):
     out = {}
     counter = [0]
 
+    def outcome(fn):
+        return _outcome(fn, tmp)
+
     def fresh():
         counter[0] += 1
         d = os.path.join(tmp, f"d{counter[0]}")
@@ -62,32 +66,32 @@ def scenarios(tmp):
         return BasicTensorAwareStateDict({"iteration": 5, "names": ["a", "b"], "nested": {"lr": 0.5}})
 
     # ---- BasicTensorAwareStateDict ---------------------------------------------------------------------------------
-    out["tasd_rejects_host_tensors"] = _outcome(lambda: BasicTensorAwareStateDict({"w": torch.zeros(2)}))
-    out["tasd_without_tensors_pops_nothing"] = _outcome(lambda: tasd().pop_tensors())
+    out["tasd_rejects_host_tensors"] = outcome(lambda: BasicTensorAwareStateDict({"w": torch.zeros(2)}))
+    out["tasd_without_tensors_pops_nothing"] = outcome(lambda: tasd().pop_tensors())
 
     def twice():
         t = tasd()
         t.pop_tensors()
         return t.pop_tensors()
 
-    out["tasd_pop_twice"] = _outcome(twice)
-    out["tasd_insert_when_not_hollow"] = _outcome(lambda: tasd().insert_tensors([]))
-    out["tasd_init_when_not_hollow"] = _outcome(lambda: tasd().init_tensors())
+    out["tasd_pop_twice"] = outcome(twice)
+    out["tasd_insert_when_not_hollow"] = outcome(lambda: tasd().insert_tensors([]))
+    out["tasd_init_when_not_hollow"] = outcome(lambda: tasd().init_tensors())
 
     def hollow(method, *args):
         t = tasd()
         t.pop_tensors()
         return getattr(t, method)(*args)
 
-    out["tasd_copy_to_cpu_when_hollow"] = _outcome(lambda: hollow("copy_tensors_to_cpu"))
-    out["tasd_restore_device_when_hollow"] = _outcome(lambda: hollow("restore_tensor_device"))
+    out["tasd_copy_to_cpu_when_hollow"] = outcome(lambda: hollow("copy_tensors_to_cpu"))
+    out["tasd_restore_device_when_hollow"] = outcome(lambda: hollow("restore_tensor_device"))
 
     def tensors_when_hollow():
         t = tasd()
         t.pop_tensors()
         return list(t.tensors)
 
-    out["tasd_tensors_when_hollow"] = _outcome(tensors_when_hollow)
+    out["tasd_tensors_when_hollow"] = outcome(tensors_when_hollow)
 
     def roundtrip():
         t = tasd()
@@ -98,13 +102,13 @@ def scenarios(tmp):
         flags.append(t.is_hollow)
         return flags, t.state_dict, list(t.tensors)
 
-    out["tasd_hollow_flags_roundtrip"] = _outcome(roundtrip)
+    out["tasd_hollow_flags_roundtrip"] = outcome(roundtrip)
 
     # ---- LocalCheckpointManager --------------------------------------------------------------------------------------
-    out["manager_load_before_find_latest"] = _outcome(lambda: LocalCheckpointManager(fresh()).load())
-    out["manager_find_latest_on_empty_directory"] = _outcome(lambda: LocalCheckpointManager(fresh()).find_latest())
-    out["manager_negative_iteration"] = _outcome(lambda: LocalCheckpointManager(fresh())._ckpt_id(-1))
-    out["manager_ckpt_id"] = _outcome(lambda: LocalCheckpointManager(fresh(), session_id="s")._ckpt_id(12))
+    out["manager_load_before_find_latest"] = outcome(lambda: LocalCheckpointManager(fresh()).load())
+    out["manager_find_latest_on_empty_directory"] = outcome(lambda: LocalCheckpointManager(fresh()).find_latest())
+    out["manager_negative_iteration"] = outcome(lambda: LocalCheckpointManager(fresh())._ckpt_id(-1))
+    out["manager_ckpt_id"] = outcome(lambda: LocalCheckpointManager(fresh(), session_id="s")._ckpt_id(12))
 
     def save_find_load():
         root = fresh()
@@ -115,14 +119,14 @@ def scenarios(tmp):
         names = sorted(os.path.relpath(os.path.join(dp, f), root) for dp, _, fs in os.walk(root) for f in fs)
         return res, latest, list(cid), loaded.state_dict, names
 
-    out["manager_sync_save_find_load"] = _outcome(save_find_load)
+    out["manager_sync_save_find_load"] = outcome(save_find_load)
 
     def other_session():
         root = fresh()
         LocalCheckpointManager(root, session_id="one").save(tasd(), 3, is_async=False)
         return LocalCheckpointManager(root, session_id="two").find_latest()
 
-    out["manager_other_session_sees_nothing"] = _outcome(other_session)
+    out["manager_other_session_sees_nothing"] = outcome(other_session)
 
     def keeps_only_latest():
         root = fresh()
@@ -134,7 +138,7 @@ def scenarios(tmp):
         time.sleep(1.0)  # removal of older iterations may run in the background
         return mgr.find_latest(), sorted(f for _, _, fs in os.walk(root) for f in fs)
 
-    out["manager_keeps_only_the_latest_iteration"] = _outcome(keeps_only_latest)
+    out["manager_keeps_only_the_latest_iteration"] = outcome(keeps_only_latest)
 
     def older_iteration():
         mgr = LocalCheckpointManager(fresh())
@@ -142,7 +146,7 @@ def scenarios(tmp):
         mgr.find_latest()  # (latest_iteration is invalid right after a save: this makes 5 known)
         return mgr.save(tasd(), 3, is_async=False)
 
-    out["manager_refuses_an_older_iteration"] = _outcome(older_iteration)
+    out["manager_refuses_an_older_iteration"] = outcome(older_iteration)
 
     def dirty_file():
         mgr = LocalCheckpointManager(fresh())
@@ -150,7 +154,7 @@ def scenarios(tmp):
         mgr._local_ckpt_path_from_id(mgr._ckpt_id(3), True).touch()
         return mgr.save(tasd(), 3, is_async=False)
 
-    out["manager_dirty_file_of_the_same_id"] = _outcome(dirty_file)
+    out["manager_dirty_file_of_the_same_id"] = outcome(dirty_file)
 
     def dirty_is_invisible_and_cleaned():
         mgr = LocalCheckpointManager(fresh())
@@ -161,7 +165,7 @@ def scenarios(tmp):
         mgr._cleanup_failed_save(3)
         return seen, sorted(p.name for p in mgr.local_ckpt_dir.iterdir())
 
-    out["manager_dirty_files_are_invisible_and_removed"] = _outcome(dirty_is_invisible_and_cleaned)
+    out["manager_dirty_files_are_invisible_and_removed"] = outcome(dirty_is_invisible_and_cleaned)
 
     def load_after_file_vanished():
         mgr = LocalCheckpointManager(fresh())
@@ -171,7 +175,7 @@ def scenarios(tmp):
             p.unlink()
         return mgr.load()
 
-    out["manager_load_after_the_file_vanished"] = _outcome(load_after_file_vanished)
+    out["manager_load_after_the_file_vanished"] = outcome(load_after_file_vanished)
 
     # ---- AsyncRequest ------------------------------------------------------------------------------------------------
     def frozen():
@@ -179,7 +183,7 @@ def scenarios(tmp):
         r2 = r.freeze()
         return r.is_frozen, r2.is_frozen, r2.add_finalize_fn(print)
 
-    out["async_request_frozen_rejects_finalize_fns"] = _outcome(frozen)
+    out["async_request_frozen_rejects_finalize_fns"] = outcome(frozen)
 
     def finalize_order():
         seen = []
@@ -189,7 +193,7 @@ def scenarios(tmp):
             fn()
         return seen
 
-    out["async_request_finalize_fns_keep_order"] = _outcome(finalize_order)
+    out["async_request_finalize_fns_keep_order"] = outcome(finalize_order)
 
     # ---- AsyncCallsQueue with a persistent worker (host functions only) -----------------------------------------------
     from nvidia_resiliency_ext.checkpointing.async_ckpt.core import AsyncCallsQueue
@@ -210,7 +214,7 @@ def scenarios(tmp):
         finally:
             q.close()
 
-    out["queue_two_requests_finalize_in_order"] = _outcome(queue_flow)
+    out["queue_two_requests_finalize_in_order"] = outcome(queue_flow)
 
     def queue_sync_request():
         d = fresh()
@@ -219,7 +223,7 @@ def scenarios(tmp):
         r.execute_sync()
         return seen, open(os.path.join(d, "s.txt")).read()
 
-    out["request_execute_sync_runs_fn_and_finalizers"] = _outcome(queue_sync_request)
+    out["request_execute_sync_runs_fn_and_finalizers"] = outcome(queue_sync_request)
 
     # ---- parse_group_sequence ----------------------------------------------------------------------------------------
     for name, kw in {
@@ -230,5 +234,5 @@ def scenarios(tmp):
         "jump1_factor4_world8": dict(replication_jump=1, replication_factor=4, world_size=8),
         "factor1": dict(replication_jump=1, replication_factor=1, world_size=4),
     }.items():
-        out[f"group_sequence_{name}"] = _outcome(lambda kw=kw: parse_group_sequence(**kw))
+        out[f"group_sequence_{name}"] = outcome(lambda kw=kw: parse_group_sequence(**kw))
     return out

@@ -1,7 +1,7 @@
 """Test configuration.
 
 * ``-m "not gpu"`` : oracle vs golden vectors, host logic (gloo, world_size 1 and 2), C-ABI symbol check.
-* ``-m gpu``       : parity of the CUDA path (through the C ABI) against the oracle, on a real B200.
+* ``-m gpu``       : parity of the CUDA path (through the C ABI) against the oracle, on a real H100.
 """
 import os
 import socket
@@ -37,7 +37,7 @@ except ImportError:  # the property tests are skipped where hypothesis is missin
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100)")
     config.addinivalue_line("markers", "multigpu: needs at least 2 CUDA devices")
 
 

@@ -28,7 +28,7 @@ import tempfile
 HERE = os.path.dirname(os.path.abspath(__file__))
 REF_SRC = "/root/reference/src"
 assert os.path.isdir(REF_SRC), "the reference tree is needed to (re)generate golden vectors"
-sys.path.insert(0, REF_SRC)  # the REFERENCE package, not the B200 mirror
+sys.path.insert(0, REF_SRC)  # the REFERENCE package, not the mirror
 
 import numpy as np  # noqa: E402
 import torch  # noqa: E402

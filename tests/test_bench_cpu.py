@@ -99,13 +99,37 @@ def _args(B, **over):
 
     ns = argparse.Namespace(gpus=1, steps=2, warmup=3, impl="engine", config="c2", narrow=False, persist_steps=1, load_reps=1, scale=1.0,
                             baseline_sample_gb=0.001, no_cpu_baseline=True, no_verify=False, no_restore=False, no_training_loop=True,
-                            no_ceiling=True, no_c3_kernel=False, traffic_bytes=None)
+                            no_ceiling=True, no_c3_kernel=False, traffic_bytes=None, dump_outputs=None)
     for k, v in over.items():
         setattr(ns, k, v)
     return ns
 
 
-def test_run_arm_assembles_the_same_config_in_both_arms(bench, monkeypatch, built_library, dist_1rank):
+def test_dump_outputs_writes_a_fixed_bounded_sample(bench, tmp_path, monkeypatch):
+    """--dump-outputs: every tensor of the saved file under its key, float32 (bf16 widened exactly), small tensors whole, large
+    ones as the same seeded sample on every run, within DUMP_BYTES."""
+    import numpy as np
+
+    B = bench
+    g = torch.Generator().manual_seed(5)
+    sd = {"model": {"w": torch.randn(300, 7, generator=g), "h": torch.randn(9, generator=g).to(torch.bfloat16)},
+          "optimizer": {"state": {0: {"step": torch.tensor(3.0)}}}}
+    torch.save(sd, tmp_path / "ckpt.pt")
+    monkeypatch.setattr(B, "DUMP_BYTES", 8 * 3 * 1000)  # 1000 elements per tensor: "w" (2100) is sampled
+    assert B.dump_outputs(tmp_path / "ckpt.pt", tmp_path / "a") == 3
+    B.dump_outputs(tmp_path / "ckpt.pt", tmp_path / "b")
+    names = sorted(p.name for p in (tmp_path / "a").iterdir())
+    assert names == ["model.h.npy", "model.w.npy", "optimizer.state.0.step.npy"]
+    for n in names:
+        a, b = np.load(tmp_path / "a" / n), np.load(tmp_path / "b" / n)
+        assert a.dtype == np.float32 and np.array_equal(a, b)
+    assert np.array_equal(np.load(tmp_path / "a" / "model.h.npy"), sd["model"]["h"].float().numpy())
+    w = np.load(tmp_path / "a" / "model.w.npy")
+    assert w.size == 1000 and np.isin(w, sd["model"]["w"].numpy().reshape(-1)).all()
+    assert sum((tmp_path / "a" / n).stat().st_size - 128 for n in names) <= B.DUMP_BYTES
+
+
+def test_run_arm_assembles_the_same_config_in_both_arms(bench, monkeypatch, built_library, dist_1rank, tmp_path):
     """The whole of run_arm (minus the GEMM loop and the PCIe ceiling, which need a GPU) on the stand-in device: the JSON line
     of both arms is assembled without error, carries the contract's keys, and `config` is identical in both (the driver
     compares it to decide whether the two arms measured the same thing)."""
@@ -119,8 +143,9 @@ def test_run_arm_assembles_the_same_config_in_both_arms(bench, monkeypatch, buil
             return sd, sum(t.numel() * t.element_size() for t in B.flatten(sd))
 
         monkeypatch.setattr(B, "llama3_8b_shard_state", state)
-        eng = B.run_arm(_args(B), 0, 1, 0)
+        eng = B.run_arm(_args(B, dump_outputs=str(tmp_path / "dump")), 0, 1, 0)
         c3 = B.run_arm(_args(B, config="c3", narrow=True, no_restore=True), 0, 1, 0)
+    assert len(list((tmp_path / "dump").glob("*.npy"))) == len(B.flatten(_small_state(False)))
     monkeypatch.setattr(B, "llama3_8b_shard_state", lambda dev, seed=0, scale=1.0: (_small_state(False), sum(t.numel() * t.element_size() for t in B.flatten(_small_state(False)))))
     ref = B.run_arm(_args(B, impl="reference", no_restore=True), 0, 1, 0)
     for line in (eng, c3, ref):

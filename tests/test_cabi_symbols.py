@@ -33,7 +33,7 @@ def test_library_loads_through_binding_and_reports_abi(built_library):
     assert "invalid" in _cabi.strerror(_cabi.E_INVALID)
 
 
-def test_library_is_sm100a_only(built_library):
+def test_library_is_sm90a_only(built_library):
     import shutil
     import subprocess
 
@@ -41,7 +41,7 @@ def test_library_is_sm100a_only(built_library):
         return
     out = subprocess.run(["cuobjdump", "-lelf", str(built_library)], capture_output=True, text=True).stdout
     archs = set(re.findall(r"sm_(\d+a?)", out))
-    assert archs == {"100a"}, archs
+    assert archs == {"90a"}, archs
 
 
 def test_no_oracle_in_product():

@@ -318,6 +318,29 @@ def test_warmup_creates_the_resources_of_the_first_save(monkeypatch, built_libra
             ckpt.close()
 
 
+def test_reserve_sizes_slots_for_a_zero_copy_save(monkeypatch, built_library, shm_dir, dist_1rank):
+    """reserve(packed bytes, tensors) leaves room for the checkpoint file's records and directory behind the payload: the
+    zero-copy save of that size that follows allocates and pins no new host buffer inside the call."""
+    from nvidia_resiliency_ext.checkpointing.async_ckpt.torch_ckpt import TorchAsyncCheckpoint
+
+    monkeypatch.setenv("NVRX_B200_ZERO_COPY", "1")
+    with fake_device(monkeypatch) as (engine, lib):
+        ckpt = TorchAsyncCheckpoint(persistent_queue=False)
+        try:
+            sd = _state(5)
+            tensors = _flat(sd)
+            engine.reserve(sum(t.numel() * t.element_size() for t in tensors) + (1 << 20), len(tensors))
+            bufs = [s.buf.name for s in engine._slots if s.buf is not None]
+            assert bufs
+            ckpt.async_save(sd, shm_dir / "r.pt")
+            ckpt.finalize_async_save(blocking=True)
+            assert [s.buf.name for s in engine._slots if s.buf is not None] == bufs
+            assert os.stat(shm_dir / "r.pt").st_nlink > 1  # published by the hard link, not copied
+            _same(torch.load(shm_dir / "r.pt", weights_only=False), _state(5, wrap=False))
+        finally:
+            ckpt.close()
+
+
 @pytest.mark.parametrize("seed,persistent", [(1, False), (2, False), (3, False), (4, True)])
 def test_random_sequences_of_saves_deletes_restores(monkeypatch, built_library, shm_dir, tmp_path, dist_1rank, seed, persistent):
     """Slot life cycle under a random workload: zero-copy and copying saves to /dev/shm and to another file system, files
@@ -509,7 +532,7 @@ def test_restoring_the_state_dict_that_was_just_saved(monkeypatch, built_library
     """Reference test_basic_local.py:62-64: after save() the caller's state dict holds host tensors -- here views of the
     snapshot slot, which is free again once the save is finalized -- and ``restore_tensor_device()`` on it must give the
     original values back.  With the container geometry of the default mode the views do not sit at the dense offsets of a
-    restore plan; gathering them into "a free slot" picked the slot they live in (found on the B200 box in round 2)."""
+    restore plan; gathering them into "a free slot" picked the slot they live in."""
     from nvidia_resiliency_ext.checkpointing.local.basic_state_dict import BasicTensorAwareStateDict
     from nvidia_resiliency_ext.checkpointing.local.ckpt_managers.local_manager import LocalCheckpointManager
 

@@ -1,5 +1,5 @@
 """Parity of the CUDA hot path (called through the C ABI) against the oracle.  Bit-exact: this is byte work.
-Run on the B200 box: ``pytest -m gpu``."""
+Run on an H100: ``pytest -m gpu``."""
 import numpy as np
 import pytest
 import torch

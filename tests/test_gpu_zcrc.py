@@ -1,6 +1,6 @@
 """GPU CRC-32 (csrc/crc_kernels.cuh) on the device.  The arithmetic, the tables and the CPU-only chaining are covered without a
 GPU (tests/test_crc_cpu.py runs the kernel's own device functions lane by lane on the host); what is left for the GPU is the
-kernel's indexing / launch and the engine plumbing.  First run on a B200 in round 2."""
+kernel's indexing / launch and the engine plumbing."""
 import ctypes as C
 import os
 import zipfile
@@ -12,7 +12,7 @@ import torch
 
 from oracle import crc_oracle as co
 
-pytestmark = pytest.mark.gpu  # validated on B200 in round 2 (profiles/r02_pytest_gpu_*.log): part of the default suite
+pytestmark = pytest.mark.gpu  # part of the default suite
 
 
 def test_kernel_values_match_zlib(built_library):

@@ -10,7 +10,7 @@ import torch.distributed.checkpoint as dcp
 from torch.distributed.checkpoint import DefaultSavePlanner, FileSystemReader, FileSystemWriter
 
 # (the writer's host side is covered by tests/test_dcp_async_cpu.py, byte for byte against the reference's own output)
-pytestmark = pytest.mark.gpu  # validated on B200 in round 2 (profiles/r02_pytest_gpu_*.log): part of the default suite
+pytestmark = pytest.mark.gpu  # part of the default suite
 
 
 def _state(step=0):

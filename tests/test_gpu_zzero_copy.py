@@ -1,13 +1,13 @@
 """Zero-copy persistence on the GPU (the default since round 2; ``NVRX_B200_ZERO_COPY=0`` opts out): the pinned slot a snapshot drains into IS the
 checkpoint file on /dev/shm (hard link), so a save is durable as soon as its drain has finished.
 
-The host half is covered on the CPU (tests/test_zero_copy_cpu.py).  First run (and made the default mode) on a B200 in round 2."""
+The host half is covered on the CPU (tests/test_zero_copy_cpu.py)."""
 import os
 
 import pytest
 import torch
 
-pytestmark = pytest.mark.gpu  # validated on B200 in round 2 (profiles/r02_pytest_gpu_*.log): part of the default suite
+pytestmark = pytest.mark.gpu  # part of the default suite
 
 
 def _state(seed, n=12):

@@ -105,20 +105,20 @@ DCP_GROUPS = ["test_async_is_equivalent_to_sync", "test_invalid_async_setup", "t
 
 def _dcp_async_writer_tests(world):
     """All 13 cases of the reference's test_async_writer.py (the last -k pattern also selects ..._followed_by_delete).  Each
-    group runs in a process of its own with its own time limit: in one process the file did not finish within 900 s on the
-    B200 box in round 2 -- its last output came about 31 s in, then nothing.  Cause not found: every group passes on its own
-    (profiles/r02_reference_dcp_tests.log), and the same 13 scenarios replayed in ONE process on the stand-in device
+    group runs in a process of its own with its own time limit: in one process the file once did not finish within 900 s
+    -- its last output came about 31 s in, then nothing.  Cause not found: every group passes on its own, and the same 13 scenarios replayed in ONE process on the stand-in device
     (queues with daemon / non-daemon workers, failing writers, caches, abort + resume) finish, so the host logic alone does
     not hang."""
     passed = 0
     for group in DCP_GROUPS:
-        out = run_reference_tests(["test_async_writer.py"], world, ["-k", group], timeout=150, retries=1)
+        # a hang guard, not a speed check: the abort group takes about 145 s on a 16-core H100 host
+        out = run_reference_tests(["test_async_writer.py"], world, ["-k", group], timeout=300, retries=1)
         assert " passed" in out and "failed" not in out, group
         passed += passed_count(out)
     assert passed == 13
 
 
-# one rank first (what a 1-GPU box runs; all green on B200 in round 2), the two-rank variants after them
+# one rank first (what a 1-GPU box runs), the two-rank variants after them
 def test_reference_async_save_tests():
     _async_save_tests(1)
 

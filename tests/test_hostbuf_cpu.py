@@ -362,7 +362,7 @@ def _save_repeatedly(path, seed, rounds):
 
 def test_several_writers_on_one_path_do_not_hurt_each_other(built_library, tmp_path):
     """The reference's own test saves the same path from every rank (tests/checkpointing/unit/test_async_save.py:38).  A writer
-    that truncates the file another one has mapped kills that one with SIGBUS (seen at world size 2 on the B200 box): every
+    that truncates the file another one has mapped kills that one with SIGBUS (seen at world size 2 on a GPU box): every
     writer fills a private file and renames it into place."""
     import multiprocessing as mp
 

@@ -1,4 +1,4 @@
-"""Times the checksum kernel (nvrx_crc_run) on a B200 with CUDA events: both table layouts, C2-shaped extents.
+"""Times the checksum kernel (nvrx_crc_run) on the GPU with CUDA events: both table layouts, C2-shaped extents.
 
     python tools/crc_bench.py [--gb 16] [--reps 7]
 Prints one JSON line per variant: GB/s over the bytes the kernel reads, fraction of the measured HBM peak, and a spot check

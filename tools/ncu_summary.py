@@ -1,6 +1,6 @@
 """Summarise an `ncu --set full` report of the walkers into profiles/<name>.json + .md (run in the build container):
 
-    python tools/ncu_summary.py gpurun_out/v2b/prof_walk.ncu-rep profiles/r02_ncu_walk_summary --commit <sha> \
+    python tools/ncu_summary.py prof_walk.ncu-rep ncu_walk_summary --commit <sha> \
         --labels "pack TMA walker (C2 bit copy)" "scatter TMA walker" "pack LDG walker" "scatter LDG walker" \
                  "pack LDG narrow fp32->bf16 (C3)" "scatter LDG widen bf16->fp32"
 """
@@ -27,6 +27,7 @@ def main():
     ap.add_argument("report")
     ap.add_argument("out_prefix")
     ap.add_argument("--commit", default="?")
+    ap.add_argument("--gpu", default="H100", help="card (and power limit) the report was captured on")
     ap.add_argument("--labels", nargs="*", default=[])
     ap.add_argument("--algorithmic", nargs="*", type=float, default=[], help="algorithmic bytes per launch, per kernel")
     args = ap.parse_args()
@@ -58,7 +59,7 @@ def main():
     doc = {"commit": args.commit, "command": f"ncu --set full --clock-control none --import-source on ... ({args.report})", "kernels": kernels}
     json.dump(doc, open(args.out_prefix + ".json", "w"), indent=1)
     with open(args.out_prefix + ".md", "w") as f:
-        f.write(f"# ncu --set full, B200, C2 state (16.06 GB, 1455 tensors), one launch each -- captured at commit {args.commit}\n\n")
+        f.write(f"# ncu --set full, {args.gpu}, C2 state (16.06 GB, 1455 tensors), one launch each -- captured at commit {args.commit}\n\n")
         f.write("| kernel | time (ms) | DRAM read (GB) | DRAM write (GB) | traffic / algorithmic | DRAM % of ncu peak | regs | grid x block |\n|---|---|---|---|---|---|---|---|\n")
         for k in kernels:
             rd = k.get("dram__bytes_read.sum", 0) * TO_BYTES.get(k.get("dram__bytes_read.sum.unit", "byte"), 1) / 1e9

@@ -8,7 +8,7 @@ checkpoint N overlaps training steps N+1, N+2, ... instead of stalling them.
 
 Prints a markdown table (one row per training step: start / end on the GPU, bytes in host memory at its end) and one JSON line.
 
-    python tools/overlap_timeline.py > profiles/r02_overlap_timeline.md
+    python tools/overlap_timeline.py > overlap_timeline.md
 """
 import ctypes as C
 import json
@@ -96,7 +96,7 @@ def main():
 
     first = next((ts for ts, v in samples if v > 0), None)
     last = next((ts for ts, v in samples if v >= packed), None)
-    print("# One checkpoint inside a running training loop: the drain overlaps the following steps (B200, C2 state, 16.06 GB)\n")
+    print(f"# One checkpoint inside a running training loop: the drain overlaps the following steps ({torch.cuda.get_device_name()}, C2 state, 16.06 GB)\n")
     print(f"training step = {loop.gemms} bf16 8192^3 GEMMs ({loop.step_ms:.1f} ms); `async_save` is called before step {steps_before}: "
           f"call took {(t_ret - t_call) * 1e3:.2f} ms on the host.\n")
     print("| step | GPU start (ms) | GPU end (ms) | duration (ms) | snapshot bytes in host memory at its end |")

@@ -4,7 +4,7 @@
 set -euo pipefail
 cd "$(dirname "$0")/.."
 SO=nvidia-resiliency-ext_b200/nvidia_resiliency_ext/checkpointing/b200/_lib/libnvrx_snap.so
-echo "# Static SASS / resource summary of libnvrx_snap.so (sm_100a), nvcc $(nvcc --version | grep -o 'V[0-9][0-9.]*' | tail -1)"
+echo "# Static SASS / resource summary of libnvrx_snap.so (sm_90a), nvcc $(nvcc --version | grep -o 'V[0-9][0-9.]*' | tail -1)"
 echo
 echo "## Resource usage (cuobjdump -res-usage): no spills (STACK:0, LOCAL:0) in any walker"
 echo
