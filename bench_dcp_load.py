@@ -1,0 +1,165 @@
+"""``python bench_dcp_load.py --gpus 1 --steps K --warmup W [--scale S]``: torch.distributed.checkpoint loads of the C2
+state (bench.py's workload), stock ``FileSystemReader`` against ``CachedMetadataFileSystemReader(load_on_engine=True)``, alternating the two, on three layouts:
+
+    same      saved by this process from the CUDA state, loaded into the same layout
+    shard0    saved as Shard(0) DTensors by 2 gloo CPU ranks, loaded into full CUDA tensors
+    shard1    saved as Shard(1) the same way (every read item is a column box: non-contiguous on the saved side)
+
+Prints one JSON line.  Per layout and arm: wall time to device sync and GB/s; for the engine arm the box-kernel time (CUDA
+events around the launches only), its
+algorithmic bytes and their share of 3.35 TB/s, the peak staging bytes; and whether every loaded tensor is bit-equal
+between the arms.  Checkpoints go to a temporary directory (``/dev/shm`` when writable) and are removed after each layout."""
+import argparse
+import json
+import os
+import shutil
+import subprocess
+import sys
+import tempfile
+import time
+from pathlib import Path
+
+ROOT = Path(__file__).resolve().parent
+for _p in (str(ROOT), str(ROOT / "nvidia-resiliency-ext_b200")):
+    if _p not in sys.path:
+        sys.path.insert(0, _p)
+
+import torch  # noqa: E402
+import torch.distributed.checkpoint as dcp  # noqa: E402
+
+HBM_GBS = 3350.0  # H100 SXM data sheet
+
+
+def _flat_state(device, scale):
+    from bench import flatten, llama3_8b_shard_state
+
+    sd, _ = llama3_8b_shard_state(device, scale=scale)
+    return {f"t{i:04d}": t for i, t in enumerate(flatten(sd))}
+
+
+def _save_sharded(rank, world, port, root, placement, scale):
+    import torch.distributed as dist
+    from torch.distributed.device_mesh import init_device_mesh
+    from torch.distributed.tensor import Replicate, Shard, distribute_tensor
+
+    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world))
+    dist.init_process_group("gloo", rank=rank, world_size=world)
+    mesh = init_device_mesh("cpu", (world,))
+    sd = {}
+    for k, v in _flat_state("cpu", scale).items():
+        pl = Shard(placement) if v.dim() > placement else (Shard(0) if v.dim() else Replicate())
+        sd[k] = distribute_tensor(v, mesh, [pl])
+    dcp.save(sd, checkpoint_id=root)
+    dist.barrier()
+    dist.destroy_process_group()
+
+
+def _card():
+    try:
+        out = subprocess.run(["nvidia-smi", "--id=0", "--query-gpu=name,power.limit", "--format=csv,noheader"],
+                             capture_output=True, text=True, timeout=30).stdout.strip()
+        name, power = [x.strip() for x in out.split(",")[:2]]
+        return name, power
+    except Exception:  # noqa: BLE001
+        return torch.cuda.get_device_name(0), "unknown"
+
+
+def _bits_equal(a, b):
+    return a.dtype == b.dtype and a.shape == b.shape and (
+        a.numel() == 0 or torch.equal(a.contiguous().view(-1).view(torch.uint8), b.contiguous().view(-1).view(torch.uint8)))
+
+
+def run(args):
+    from nvidia_resiliency_ext.checkpointing.async_ckpt.cached_metadata_filesystem_reader import CachedMetadataFileSystemReader
+    from nvidia_resiliency_ext.checkpointing.b200.engine import SnapshotEngine
+
+    import torch.multiprocessing as mp
+
+    local = 0
+    torch.cuda.set_device(local)
+
+    base = "/dev/shm" if os.access("/dev/shm", os.W_OK) else None
+    like = _flat_state("cuda", args.scale)
+    total = sum(t.nbytes for t in like.values())
+    engine = SnapshotEngine.get(local)
+    engine.timing = True  # box-kernel time from CUDA events around every launch
+    card, power = _card()
+    layouts = {}
+    for layout in ("same", "shard0", "shard1"):
+        root = tempfile.mkdtemp(dir=base, prefix=f"nvrx_dcp_load_{layout}_")
+        try:
+            if layout == "same":
+                dcp.save(like, checkpoint_id=root)
+            else:
+                ctx = mp.get_context("spawn")
+                port = 29600 + (os.getpid() % 200)
+                procs = [ctx.Process(target=_save_sharded, args=(r, 2, port, root, int(layout[-1]), args.scale)) for r in range(2)]
+                for p in procs:
+                    p.start()
+                for p in procs:
+                    p.join()
+                assert all(p.exitcode == 0 for p in procs), [p.exitcode for p in procs]
+            outs = {arm: {k: torch.empty_like(v) for k, v in like.items()} for arm in ("stock", "engine")}
+            times = {"stock": [], "engine": []}
+            box_ms, stats = [], None
+            for it in range(args.warmup + args.steps):
+                for arm in ("stock", "engine"):
+                    reader = (dcp.FileSystemReader(root) if arm == "stock"
+                              else CachedMetadataFileSystemReader(root, load_on_engine=True))
+                    torch.cuda.synchronize()
+                    t0 = time.perf_counter()
+                    dcp.load(outs[arm], storage_reader=reader)
+                    torch.cuda.synchronize()
+                    dt = time.perf_counter() - t0
+                    if it >= args.warmup:
+                        times[arm].append(dt)
+                        if arm == "engine":
+                            stats = dict(engine.last_box_load)
+                            box_ms.append(stats["box_ms"])
+            CachedMetadataFileSystemReader.clear_metadata_cache()
+            med = {arm: sorted(v)[len(v) // 2] for arm, v in times.items()}
+            kms = sorted(box_ms)[len(box_ms) // 2]
+            layouts[layout] = {
+                "stock_s": round(med["stock"], 4),
+                "stock_GBps": round(total / med["stock"] / 1e9, 3),
+                "engine_s": round(med["engine"], 4),
+                "engine_GBps": round(total / med["engine"] / 1e9, 3),
+                "box_kernel_ms": round(kms, 3),
+                "box_algorithmic_bytes": stats["algorithmic_bytes"],
+                "box_share_of_3p35TBps": round(stats["algorithmic_bytes"] / (kms * 1e-3) / (HBM_GBS * 1e9), 4) if kms else None,
+                "box_batches": stats["batches"],
+                "peak_staging_bytes": stats["peak_staging_bytes"],
+                "bits_equal": all(_bits_equal(outs["stock"][k], outs["engine"][k]) for k in like),
+            }
+            del outs
+        finally:
+            shutil.rmtree(root, ignore_errors=True)
+    return {
+        "metric": "dcp_load_GBps",
+        "value": layouts["same"]["engine_GBps"],
+        "unit": "GB/s",
+        "config": {"workload": f"C2 state ({total / 1e9:.2f} GB, scale {args.scale}) through dcp.save / dcp.load",
+                   "steps": args.steps, "warmup": args.warmup, "staging_budget_bytes": SnapshotEngine.DCP_LOAD_STAGING},
+        "gpu": card,
+        "power_limit": power,
+        "layouts": layouts,
+        "bits_equal": all(v["bits_equal"] for v in layouts.values()),
+    }
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--gpus", type=int, default=1, help="one GPU only (the loads run in this process)")
+    ap.add_argument("--steps", type=int, default=3, help="timed loads per layout and arm")
+    ap.add_argument("--warmup", type=int, default=1)
+    ap.add_argument("--scale", type=float, default=1.0, help="shrink the state (numbers at != 1.0 are not C2)")
+    args = ap.parse_args()
+    if args.gpus != 1:
+        ap.error("dcp-load runs on one GPU (--gpus 1)")
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_dcp_load.py needs a CUDA device (the engine load path has no CPU fallback)")
+    print(json.dumps(run(args)), flush=True)
+
+
+if __name__ == "__main__":
+    main()

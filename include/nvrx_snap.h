@@ -30,7 +30,7 @@
 extern "C" {
 #endif
 
-#define NVRX_ABI_VERSION 2
+#define NVRX_ABI_VERSION 3
 
 enum {
     NVRX_OK = 0,
@@ -160,6 +160,48 @@ int nvrx_fill(void* staging, const void* host_src, uint64_t bytes, uint64_t chun
 int nvrx_fill_from_fd(void* staging, uint64_t staging_bytes, int fd, int64_t n, const uint64_t* stg_offs,
                       const uint64_t* nbytes, const uint64_t* file_offs, uint64_t chunk_bytes, int ring_slots, int threads,
                       int device, void* stream);
+
+/* ---- box scatter: resharded torch.distributed.checkpoint loads --------------------------------
+ * Replaces the per-item tail of torch's FileSystemReader.read_data (torch/distributed/checkpoint/filesystem.py:897-915:
+ * torch.load of the whole saved chunk, narrow_tensor_by_index, target.copy_() into a possibly non-contiguous view).  Each
+ * of the n boxes is an N-d sub-box of a saved chunk that already sits in device staging, written into an N-d sub-box of
+ * its destination; ONE kernel walks all of them.
+ *   elem_bytes[i]   element size of box i: 1, 2, 4, 8 or 16
+ *   ndim[i]         dims of box i, 0..NVRX_BOX_MAXDIM; sizes / strides of box i follow those of box i-1 in the flat arrays
+ *   sizes[]         extents (>= 0)
+ *   src_offs[i]     staging byte offset of element (0, ..., 0) of box i
+ *   src_strides[]   staging strides in ELEMENTS (as torch reports them, >= 0)
+ *   dst_ptrs[i]     device address of element (0, ..., 0) of the destination view of box i (NULL iff the box is empty)
+ *   dst_strides[]   destination strides in elements (>= 0; 0 only on dims of size 1)
+ *   staging_bytes   every source byte must lie below it
+ *   tile_bytes      work granule (0 = default 32 KiB; power of two in [4096, 65536])
+ * The planner drops size-1 dims, merges dims that are contiguous on both sides and, when the innermost dim is contiguous
+ * on both sides, copies whole "runs" with the vector copy of nvrx_scatter; otherwise it moves one element per thread.  A
+ * tile is (box, first row, rows, byte range): descriptors grow with boxes + tiles, not with rows.  No CUDA call is made
+ * by create / info / tiles / box. */
+#define NVRX_BOX_MAXDIM 8
+typedef struct nvrx_boxplan nvrx_boxplan;
+int nvrx_boxplan_create(int64_t n, const uint32_t* elem_bytes, const int32_t* ndim, const int64_t* sizes,
+                        const uint64_t* src_offs, const int64_t* src_strides, const void* const* dst_ptrs,
+                        const int64_t* dst_strides, uint64_t staging_bytes, uint32_t tile_bytes, int device,
+                        nvrx_boxplan** out);
+int nvrx_boxplan_destroy(nvrx_boxplan* plan);
+/* tiles of one launch / algorithmic HBM bytes of it (2 x the bytes moved) */
+int nvrx_boxplan_info(const nvrx_boxplan* plan, uint64_t* n_tiles, uint64_t* algorithmic_bytes);
+/* Introspection (tests, tooling), like nvrx_plan_tiles: tile t covers rows [row[t], row[t] + nrows[t]) of box box[t]; with
+ * one row it covers bytes [byte_off[t], byte_off[t] + nbytes[t]) of it, with several the whole rows.  Up to `capacity`
+ * entries are written (any array may be NULL). */
+int nvrx_boxplan_tiles(const nvrx_boxplan* plan, uint64_t* n_tiles, uint32_t* box, uint64_t* row, uint64_t* nrows,
+                       uint64_t* byte_off, uint32_t* nbytes, uint64_t capacity);
+/* The row geometry the planner made of box i: row r (mixed radix over sizes[0..n_outer), outermost first) is the
+ * row_bytes bytes at staging offset src_off + sum idx_d * src_stride[d] and at device address dst + sum idx_d * dst_stride[d]
+ * (byte strides).  Arrays hold NVRX_BOX_MAXDIM entries. */
+int nvrx_boxplan_box(const nvrx_boxplan* plan, int64_t i, uint64_t* row_bytes, uint32_t* n_outer, uint64_t* sizes,
+                     int64_t* src_stride, int64_t* dst_stride, uint64_t* src_off, uint64_t* dst);
+/* Upload the descriptor tables on `stream` (otherwise done by the first nvrx_box_scatter), e.g. to time the kernel alone. */
+int nvrx_boxplan_commit(nvrx_boxplan* plan, void* stream);
+/* staging -> destination views, ONE kernel launch on `stream` (grid sized from the SM count). */
+int nvrx_box_scatter(nvrx_boxplan* plan, const void* staging, void* stream);
 
 /* ---- device staging / stream helpers (so callers need no CUDA binding of their own) ---------- */
 int nvrx_dev_alloc(int device, uint64_t bytes, void** out); /* cudaMalloc, zero-filled, IPC-capable */

@@ -12,7 +12,7 @@ import os
 from pathlib import Path
 from typing import Optional
 
-ABI_VERSION = 2
+ABI_VERSION = 3
 
 OK = 0
 E_INVALID = 1000
@@ -51,6 +51,13 @@ EXPORTED_SYMBOLS = (
     "nvrx_plan_last_launches",
     "nvrx_fill",
     "nvrx_fill_from_fd",
+    "nvrx_boxplan_create",
+    "nvrx_boxplan_destroy",
+    "nvrx_boxplan_info",
+    "nvrx_boxplan_tiles",
+    "nvrx_boxplan_box",
+    "nvrx_boxplan_commit",
+    "nvrx_box_scatter",
     "nvrx_dev_alloc",
     "nvrx_dev_free",
     "nvrx_stream_create",
@@ -115,6 +122,7 @@ _u64 = C.c_uint64
 _i64 = C.c_int64
 _u32 = C.c_uint32
 _int = C.c_int
+_i32 = C.c_int32
 
 
 def _declare(lib: C.CDLL) -> None:
@@ -142,6 +150,15 @@ def _declare(lib: C.CDLL) -> None:
         "nvrx_plan_last_launches": (_int, [_vp, P(_u32)]),
         "nvrx_fill": (_int, [_vp, _vp, _u64, _u64, _vp, _vp]),
         "nvrx_fill_from_fd": (_int, [_vp, _u64, _int, _i64, P(_u64), P(_u64), P(_u64), _u64, _int, _int, _int, _vp]),
+        "nvrx_boxplan_create": (
+            _int, [_i64, P(_u32), P(_i32), P(_i64), P(_u64), P(_i64), P(_vp), P(_i64), _u64, _u32, _int, P(_vp)]
+        ),
+        "nvrx_boxplan_destroy": (_int, [_vp]),
+        "nvrx_boxplan_info": (_int, [_vp, P(_u64), P(_u64)]),
+        "nvrx_boxplan_tiles": (_int, [_vp, P(_u64), P(_u32), P(_u64), P(_u64), P(_u64), P(_u32), _u64]),
+        "nvrx_boxplan_box": (_int, [_vp, _i64, P(_u64), P(_u32), P(_u64), P(_i64), P(_i64), P(_u64), P(_u64)]),
+        "nvrx_boxplan_commit": (_int, [_vp, _vp]),
+        "nvrx_box_scatter": (_int, [_vp, _vp, _vp]),
         "nvrx_dev_alloc": (_int, [_int, _u64, P(_vp)]),
         "nvrx_dev_free": (_int, [_int, _vp]),
         "nvrx_stream_create": (_int, [_int, _int, P(_vp)]),

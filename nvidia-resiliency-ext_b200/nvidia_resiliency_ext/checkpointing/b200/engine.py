@@ -27,7 +27,7 @@ import re
 import threading
 import uuid
 from dataclasses import dataclass, field
-from typing import Dict, List, Optional, Sequence, Tuple
+from typing import Dict, List, NamedTuple, Optional, Sequence, Tuple
 
 import torch
 
@@ -276,6 +276,96 @@ class CrcPlan:
             self.close()
         except Exception:
             pass
+
+
+class BoxPlan:
+    """N-d sub-boxes of chunks in device staging -> N-d sub-boxes of destination views (``nvrx_boxplan_*``), one launch.
+    ``boxes[i] = (elem_bytes, sizes, staging byte offset of element 0, staging strides, destination address, destination
+    strides)``, strides in elements.  Creating it is CUDA-free."""
+
+    def __init__(self, boxes: Sequence[tuple], staging_bytes: int, *, device: int, tile_bytes: int = 0):
+        self._lib = _cabi.lib()
+        self._h = C.c_void_p()
+        n = len(boxes)
+        dims = [len(b[1]) for b in boxes]
+        flat = lambda k: [int(v) for b in boxes for v in b[k]]  # noqa: E731
+        i64 = lambda vals: (C.c_int64 * max(len(vals), 1))(*vals)  # noqa: E731
+        check(
+            self._lib.nvrx_boxplan_create(
+                n, _u32_array([b[0] for b in boxes]), (C.c_int32 * max(n, 1))(*dims), i64(flat(1)),
+                _u64_array([b[2] for b in boxes]), i64(flat(3)), _ptr_array([b[4] for b in boxes]), i64(flat(5)),
+                staging_bytes, tile_bytes, device, C.byref(self._h),
+            ),
+            "nvrx_boxplan_create",
+        )
+        tiles, algo = C.c_uint64(), C.c_uint64()
+        check(self._lib.nvrx_boxplan_info(self._h, C.byref(tiles), C.byref(algo)), "nvrx_boxplan_info")
+        self.n_tiles = tiles.value
+        self.algorithmic_bytes = algo.value
+
+    def tiles(self) -> List[Tuple[int, int, int, int, int]]:
+        """[(box, row, nrows, byte_off, nbytes), ...] -- the work-list as the kernel walks it (no CUDA involved)."""
+        n = self.n_tiles
+        box, nby = (C.c_uint32 * max(n, 1))(), (C.c_uint32 * max(n, 1))()
+        row, nrows, off = (C.c_uint64 * max(n, 1))(), (C.c_uint64 * max(n, 1))(), (C.c_uint64 * max(n, 1))()
+        check(self._lib.nvrx_boxplan_tiles(self._h, None, box, row, nrows, off, nby, n), "nvrx_boxplan_tiles")
+        return [(box[i], row[i], nrows[i], off[i], nby[i]) for i in range(n)]
+
+    def commit(self, stream: int) -> None:
+        check(self._lib.nvrx_boxplan_commit(self._h, stream), "nvrx_boxplan_commit")
+
+    def scatter(self, staging_ptr: int, stream: int) -> None:
+        check(self._lib.nvrx_box_scatter(self._h, staging_ptr, stream), "nvrx_box_scatter")
+
+    def close(self) -> None:
+        if self._h:
+            self._lib.nvrx_boxplan_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class BoxLoad(NamedTuple):
+    """One read of a resharded load: the sub-box of a saved chunk that lands in ``target``.
+
+    ``file_off`` / ``file_len``: where the chunk's storage bytes sit in ``path``; ``src_offset`` / ``src_strides``: element
+    offset of the sub-box's first element in that storage and the chunk's strides (elements).  The box's sizes are
+    ``target.shape``."""
+
+    path: str
+    file_off: int
+    file_len: int
+    src_offset: int
+    src_strides: Tuple[int, ...]
+    target: torch.Tensor
+
+
+def box_span(sizes: Sequence[int], strides: Sequence[int], elem: int) -> int:
+    """Bytes from a box's first element to the end of its last one (0 for an empty box); strides >= 0."""
+    if any(s == 0 for s in sizes):
+        return 0
+    return elem + sum((n - 1) * st * elem for n, st in zip(sizes, strides))
+
+
+def split_box(sizes, src_off, sstr, dst_off, dstr, elem: int, limit: int):
+    """Cut a box whose source span exceeds ``limit`` bytes along its outermost dim of size > 1 (recursively inward, so a
+    single run ends up cut into element ranges).  Yields ``(sizes, src_off, dst_off)`` pieces, offsets in elements."""
+    sizes = list(sizes)
+    if box_span(sizes, sstr, elem) <= limit:
+        yield sizes, src_off, dst_off
+        return
+    d = next(k for k, n in enumerate(sizes) if n > 1)
+    n = sizes[d]
+    rest = box_span(sizes[:d] + [1] + sizes[d + 1:], sstr, elem)
+    step = sstr[d] * elem
+    k = n if step == 0 else ((limit - rest) // step + 1 if limit >= rest else 0)
+    for i in range(0, n, max(k, 1)):
+        sub = sizes[:d] + [min(max(k, 1), n - i)] + sizes[d + 1:]
+        yield from split_box(sub, src_off + i * sstr[d], sstr, dst_off + i * dstr[d], dstr, elem, limit)
 
 
 def finish_crcs(offsets: Sequence[int], nbytes: Sequence[int], values_ptr: int, n_values: int, host_base: int) -> List[int]:
@@ -660,6 +750,9 @@ class SnapshotEngine:
         self.launches = 0  # kernels launched by this engine (pack + scatter)
         self.resident_restores = 0  # restores that read a published slot in place (no host copy)
         self.file_restores = 0  # restores fed straight from the checkpoint file through the pinned ring
+        self.box_loads = 0  # load_boxes() calls (torch.distributed.checkpoint loads on the engine)
+        self.box_batches = 0  # staging batches of those loads (one box-scatter launch each)
+        self.last_box_load: Optional[dict] = None  # batches / peak staging / algorithmic bytes (/ kernel ms) of the last one
         self._aux: Optional[Stream] = None  # checksum kernels (created on first use)
         self._pid = os.getpid()  # forked writers inherit this object; only the creator may tear it down
         # NVRX_B200_TRACE=1: host-side time stamps of the last snapshot() (enter / planned / launched), for the stall breakdown
@@ -1112,6 +1205,114 @@ class SnapshotEngine:
         if self.trace is not None:
             self.trace["restore"] = {"plan_s": t1 - t0, "staging_s": t2 - t1, "file_to_device_s": t3 - t2, "scatter_s": _time.perf_counter() - t3}
         return out
+
+    # staging bytes one batch of load_boxes() may use (the buffer is reused by every batch)
+    DCP_LOAD_STAGING = int(os.environ.get("NVRX_B200_DCP_LOAD_STAGING_MB", "2048")) << 20
+
+    def load_boxes(self, entries: Sequence[BoxLoad]) -> None:
+        """Resharded load: write the sub-box of a saved chunk described by every entry into its target view (a CUDA tensor of
+        this device, any strides, the chunk's dtype).  Blocking, like ``restore``.
+
+        Only the byte span of each sub-box is read, by ``nvrx_fill_from_fd`` (file -> pinned ring -> staging, one call per
+        file per batch) to a staging position with the same address mod 16 as the target's first byte, so that same-layout
+        loads are aligned 16-byte copies; one ``nvrx_box_scatter`` per batch writes the views.  Batches hold at most
+        ``DCP_LOAD_STAGING`` bytes and reuse one buffer: batch k+1's copies are enqueued on the stream after batch k's
+        scatter.  An entry larger than a batch is cut along its outermost dim (down to element ranges of a single run)."""
+        import time as _time
+
+        budget = max(int(self.DCP_LOAD_STAGING), 4096)
+        # pieces: (path, file offset of the span, span bytes, box tuple without staging offset, target address)
+        pieces = []
+        for e in entries:
+            t = e.target
+            if not (t.is_cuda and t.get_device() == self.device):
+                raise ValueError("load_boxes: every target must be a CUDA tensor of the engine's device")
+            elem = t.element_size()
+            sizes, dstr = list(t.shape), list(t.stride())
+            sstr = list(e.src_strides)
+            if len(sstr) != len(sizes):
+                raise ValueError(f"load_boxes: {len(sizes)}-d target for a {len(sstr)}-d source box")
+            span = box_span(sizes, sstr, elem)
+            if span and (e.src_offset < 0 or e.src_offset * elem + span > e.file_len):
+                raise ValueError(f"load_boxes: box reaches past the saved chunk in {e.path}")
+            if span == 0:
+                continue
+            for sz, so, do in split_box(sizes, e.src_offset, sstr, 0, dstr, elem, budget - 16):
+                dst = t.data_ptr() + do * elem
+                pieces.append((e.path, e.file_off + so * elem, box_span(sz, sstr, elem), (elem, sz, sstr, dst, dstr)))
+        # one nvrx_fill_from_fd per file per batch copies each ring chunk from its file's first to its last byte in it, gaps
+        # included: the pieces of a file must occupy one staging range of their own, so they are placed file by file (and in
+        # file order, which also keeps the reads sequential)
+        pieces.sort(key=lambda pc: (pc[0], pc[1]))
+        # batches: a piece starts at the first position >= the cursor that is congruent to its target address mod 16
+        batches, cur = [[]], 0
+        for piece in pieces:
+            pos = cur + (piece[3][3] - cur) % 16
+            if batches[-1] and pos + piece[2] > budget:
+                batches.append([])
+                pos = piece[3][3] % 16
+            batches[-1].append((pos,) + piece)
+            cur = pos + piece[2]
+        batches = [b for b in batches if b]
+        peak = max((b[-1][0] + b[-1][3] for b in batches), default=0)
+        stats = {"batches": len(batches), "peak_staging_bytes": peak, "algorithmic_bytes": 0, "box_ms": 0.0 if self.timing else None}
+        self.box_loads += 1
+        self.last_box_load = stats
+        if not batches:
+            return
+        staging = self._ensure_staging(peak)
+        stream = self._current_stream()
+        if self._staging_free is not None:
+            stream_wait_event(stream, self._staging_free)
+        threads = self.RESTORE_THREADS or max(self.prefault_threads, min(32, os.cpu_count() or 1))
+        fds: Dict[str, int] = {}
+        plans, timers = [], []
+        t0 = _time.perf_counter()
+        try:
+            for batch in batches:
+                by_file: Dict[str, list] = {}
+                for pos, path, file_off, nbytes, _ in batch:
+                    by_file.setdefault(path, []).append((pos, nbytes, file_off))
+                end = batch[-1][0] + batch[-1][3]
+                for path, ext in by_file.items():
+                    fd = fds.get(path)
+                    if fd is None:
+                        fd = fds[path] = os.open(path, os.O_RDONLY)
+                    check(
+                        self.lib.nvrx_fill_from_fd(
+                            staging.ptr, end, fd, len(ext), _u64_array([x[0] for x in ext]), _u64_array([x[1] for x in ext]),
+                            _u64_array([x[2] for x in ext]), self.RESTORE_CHUNK, self.RESTORE_RING, threads, self.device, stream,
+                        ),
+                        "nvrx_fill_from_fd",
+                    )
+                plan = BoxPlan(
+                    [(b[0], b[1], pos, b[2], b[3], b[4]) for pos, _, _, _, b in batch], end, device=self.device,
+                )
+                plans.append(plan)
+                stats["algorithmic_bytes"] += plan.algorithmic_bytes
+                if self.timing:
+                    plan.commit(stream)  # descriptor upload outside the timed window: the events bracket the kernel
+                    ev = (Event(self.device, timing=True), Event(self.device, timing=True))
+                    ev[0].record(stream)
+                plan.scatter(staging.ptr, stream)
+                if self.timing:
+                    ev[1].record(stream)
+                    timers.append(ev)
+                self.launches += 1 if plan.n_tiles else 0
+                self.box_batches += 1
+            done = Event(self.device)
+            done.record(stream)
+            self._staging_free = done
+            done.synchronize()
+        finally:
+            for fd in fds.values():
+                os.close(fd)
+        for plan in plans:
+            plan.close()
+        if timers:
+            stats["box_ms"] = sum(a.elapsed_ms(b) for a, b in timers)
+        if self.trace is not None:
+            self.trace["load_boxes"] = {"wall_s": _time.perf_counter() - t0}
 
     def resident_source(self, path, host_tensors: Sequence[torch.Tensor]) -> Optional[Tuple[_Slot, List[int]]]:
         """``(slot, payload offsets)`` when the checkpoint file ``path`` is a hard link to one of this engine's live,

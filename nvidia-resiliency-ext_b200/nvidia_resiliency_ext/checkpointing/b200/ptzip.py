@@ -511,13 +511,127 @@ def record_crcs(path, n_storages: int) -> Optional[List[int]]:
 
     try:
         with zipfile.ZipFile(path) as zf:
-            by_key = {}
-            for info in zf.infolist():
-                head, sep, key = info.filename.rpartition("/data/")
-                if sep and key.isdigit() and "/" not in head:
-                    by_key[int(key)] = info.CRC
+            by_key = {k: info.CRC for k, info in _data_records(zf).items()}
     except (OSError, zipfile.BadZipFile):
         return None
     if sorted(by_key) != list(range(n_storages)):
         return None
     return [by_key[i] for i in range(n_storages)]
+
+
+def _data_records(zf) -> dict:
+    """``{k: ZipInfo}`` of the storage records ``<archive>/data/<k>`` of an open ``zipfile.ZipFile`` (zip64 included)."""
+    by_key = {}
+    for info in zf.infolist():
+        head, sep, key = info.filename.rpartition("/data/")
+        if sep and key.isdigit() and "/" not in head:
+            by_key[int(key)] = info
+    return by_key
+
+
+class _FileWindow(io.RawIOBase):
+    """Read-only, seekable view of ``[offset, offset + length)`` of an open file descriptor (positional reads only)."""
+
+    def __init__(self, fd: int, offset: int, length: int):
+        self._fd, self._off, self._len, self._pos = fd, offset, length, 0
+
+    def readable(self):
+        return True
+
+    def seekable(self):
+        return True
+
+    def tell(self):
+        return self._pos
+
+    def seek(self, pos, whence=0):
+        self._pos = {0: pos, 1: self._pos + pos, 2: self._len + pos}[whence]
+        return self._pos
+
+    def readinto(self, b):
+        n = max(0, min(len(b), self._len - self._pos))
+        data = os.pread(self._fd, n, self._off + self._pos) if n else b""
+        b[: len(data)] = data
+        self._pos += len(data)
+        return len(data)
+
+
+@dataclass
+class SavedChunk:
+    """What ``torch.load`` would rebuild from one embedded tensor archive, without its payload."""
+
+    data_off: int  # file offset of the storage's first byte (the ``data/0`` record)
+    dtype: torch.dtype
+    numel: int  # elements of the storage
+    storage_offset: int
+    size: Tuple[int, ...]
+    stride: Tuple[int, ...]
+
+
+class _TensorRecordUnpickler(pickle.Unpickler):
+    """Reads the ``data.pkl`` of a single-tensor archive and executes nothing: only ``_rebuild_tensor_v2`` / ``_v3``, the
+    typed-storage classes, ``torch.<dtype>`` and an empty ``OrderedDict`` (backward hooks) are known names, and all of them
+    resolve to stand-ins that record their arguments."""
+
+    _STORAGE_DTYPES = {name: dt for dt, name in torch.storage._dtype_to_storage_type_map().items()}
+
+    def find_class(self, module, name):
+        if module == "torch._utils" and name in ("_rebuild_tensor_v2", "_rebuild_tensor_v3"):
+            return lambda storage, offset, size, stride, *rest: ("tensor", name, storage, offset, tuple(size), tuple(stride), rest)
+        if module == "collections" and name == "OrderedDict":
+            return lambda *a: ("hooks",) + a
+        if module == "torch" and name in self._STORAGE_DTYPES:
+            return ("typed", self._STORAGE_DTYPES[name])
+        if module == "torch.storage" and name == "UntypedStorage":
+            return ("typed", torch.uint8)
+        if module == "torch" and isinstance(getattr(torch, name, None), torch.dtype):
+            return ("dtype", getattr(torch, name))
+        raise pickle.UnpicklingError(f"unexpected global {module}.{name} in a tensor record")
+
+    def persistent_load(self, pid):
+        if not (isinstance(pid, tuple) and len(pid) == 5 and pid[0] == "storage" and isinstance(pid[1], tuple)):
+            raise pickle.UnpicklingError(f"unexpected persistent id {pid!r}")
+        return ("storage", pid[1][1], str(pid[2]), int(pid[4]))
+
+
+def read_tensor_record(fd: int, offset: int, length: int) -> SavedChunk:
+    """Describe the ``torch.save`` archive of ONE tensor embedded at ``[offset, offset + length)`` of ``fd`` (how
+    ``torch.distributed.checkpoint`` stores every tensor item of a ``.distcp`` file): where its payload starts, its dtype,
+    element count, storage offset, size and stride (any strides: a chunk that was not cloned keeps them).  Reads the
+    directory and ``data.pkl`` only -- not the payload -- and never runs code from the pickle; ``ValueError`` when the
+    window is not such an archive."""
+    import zipfile
+
+    try:
+        with zipfile.ZipFile(_FileWindow(fd, offset, length)) as zf:
+            recs = _data_records(zf)
+            pkl = [i for i in zf.infolist() if i.filename.endswith("/data.pkl") and i.filename.count("/") == 1]
+            if len(pkl) != 1:
+                raise ValueError("no data.pkl record")
+            rec = _TensorRecordUnpickler(io.BytesIO(zf.read(pkl[0]))).load()
+            if not (isinstance(rec, tuple) and rec[0] == "tensor" and rec[2][0] == "storage"):
+                raise ValueError("data.pkl does not describe a single tensor")
+            _, fn, (_, st_dtype, key, st_numel), st_off, size, stride, rest = rec
+            dtype = st_dtype
+            if fn == "_rebuild_tensor_v3":
+                dts = [r[1] for r in rest if isinstance(r, tuple) and r and r[0] == "dtype"]
+                if len(dts) != 1:
+                    raise ValueError("_rebuild_tensor_v3 record without a dtype")
+                dtype = dts[0]
+                elem = torch.empty(0, dtype=dtype).element_size()
+                st_numel //= elem  # an untyped storage counts bytes
+            if not key.isdigit() or int(key) not in recs:
+                raise ValueError(f"storage record data/{key} missing")
+            info = recs[int(key)]
+            if info.file_size < st_numel * torch.empty(0, dtype=dtype).element_size():
+                raise ValueError("storage record shorter than its storage")
+            if info.compress_type != zipfile.ZIP_STORED:
+                raise ValueError("compressed storage record")
+            hdr = os.pread(fd, 30, offset + info.header_offset)
+            if len(hdr) != 30 or hdr[:4] != b"PK\x03\x04":
+                raise ValueError("bad local header of the storage record")
+            name_len, extra_len = struct.unpack_from("<HH", hdr, 26)
+            data_off = offset + info.header_offset + 30 + name_len + extra_len
+    except (zipfile.BadZipFile, pickle.UnpicklingError, EOFError, TypeError, IndexError) as e:
+        raise ValueError(f"not a single-tensor torch.save archive: {e}") from e
+    return SavedChunk(data_off=data_off, dtype=dtype, numel=int(st_numel), storage_offset=int(st_off), size=size, stride=stride)
