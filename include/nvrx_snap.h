@@ -13,6 +13,10 @@
  *     >= 1000 = one of the NVRX_E_* codes.  Nothing throws.  nvrx_strerror() decodes.
  *   - the caller owns every data buffer; a plan owns only its descriptor tables.
  *   - a plan is thread-compatible (one thread at a time); there is no global mutable state.
+ *   - every call may pass its own stream.  A call that re-uploads a plan's descriptor tables (after update_ptrs, or a
+ *     change between sharded and plain packing) orders that upload after the plan's earlier kernel launches on the
+ *     device, whatever streams they ran on; the host does not wait.  A launch still queued on one stream therefore
+ *     packs or scatters the tensors the plan pointed at when it was issued.  Destroying a plan waits for its last launch.
  *
  * Packed ("staging") layout produced by a plan -- the oracle (oracle/snapshot_oracle.py) restates it:
  *   segment i (tensor i in TensorAwareStateDict flattening order, basic_state_dict.py:34-41,112-120)

@@ -79,6 +79,7 @@ struct nvrx_plan {
     bool segs_dirty = true, tiles_dirty = true;
     std::vector<cudaEvent_t> chunk_events;  // pack -> drain hand-off of the pipelined snapshot
     cudaEvent_t upload_done = nullptr;      // last H2D of the descriptor mirrors (they are reused)
+    cudaEvent_t last_launch = nullptr;      // last kernel launch that reads the device mirrors, on whichever stream it ran
     uint32_t last_launches = 0;             // kernel launches of the last nvrx_snapshot (its pack groups)
 };
 
@@ -215,6 +216,12 @@ int upload(nvrx_plan* p, cudaStream_t st) {
     // the pinned mirrors are about to be rewritten: an earlier upload must have finished reading them
     if (p->upload_done) NVRX_CUDA(cudaEventSynchronize(p->upload_done));
     else NVRX_CUDA(cudaEventCreateWithFlags(&p->upload_done, cudaEventDisableTiming));
+    // the device mirrors are about to be rewritten or freed: a launch queued earlier, possibly on another stream (a cached
+    // plan re-pointed with update_ptrs and launched on a new stream), must have read them first.  The H2D waits on the
+    // device; only freeing them for a larger table waits on the host.
+    if (p->last_launch) NVRX_CUDA(cudaStreamWaitEvent(st, p->last_launch, 0));
+    const bool grow = (p->segs_dirty && static_cast<size_t>(p->n) > p->segs_cap) || (p->tiles_dirty && p->n_tiles > p->tiles_cap);
+    if (grow && p->last_launch) NVRX_CUDA(cudaEventSynchronize(p->last_launch));
     if (p->segs_dirty && p->n > 0) {
         const size_t n = static_cast<size_t>(p->n);
         if (n > p->segs_cap) {
@@ -285,8 +292,7 @@ int launch_tma(nvrx_plan* p, const TileSpan& span, uint8_t* staging, const PeerM
 }
 
 template <int DIR>
-int launch_span(nvrx_plan* p, const TileSpan& span, uint8_t* staging, const PeerMap& pm, cudaStream_t st) {
-    if (span.na + span.nb == 0) return NVRX_OK;
+int launch_walker(nvrx_plan* p, const TileSpan& span, uint8_t* staging, const PeerMap& pm, cudaStream_t st) {
     int variant = p->variant;
     if (variant == NVRX_VARIANT_AUTO) variant = (p->any_narrow || p->n_bulk == 0) ? NVRX_VARIANT_LDG : NVRX_VARIANT_TMA;
     if (variant == NVRX_VARIANT_TMA) {
@@ -304,6 +310,17 @@ int launch_span(nvrx_plan* p, const TileSpan& span, uint8_t* staging, const Peer
     grid = std::max<uint32_t>(1, std::min(grid, span.na + span.nb));
     nvrx::walk_ldg<DIR><<<grid, nvrx::kLdgThreads, 0, st>>>(p->d_segs, span, staging, pm);
     NVRX_CUDA(cudaGetLastError());
+    return NVRX_OK;
+}
+
+// every launch is remembered in last_launch, which the next upload (on any stream) waits for
+template <int DIR>
+int launch_span(nvrx_plan* p, const TileSpan& span, uint8_t* staging, const PeerMap& pm, cudaStream_t st) {
+    if (span.na + span.nb == 0) return NVRX_OK;
+    int rc = launch_walker<DIR>(p, span, staging, pm, st);
+    if (rc) return rc;
+    if (!p->last_launch) NVRX_CUDA(cudaEventCreateWithFlags(&p->last_launch, cudaEventDisableTiming));
+    NVRX_CUDA(cudaEventRecord(p->last_launch, st));
     return NVRX_OK;
 }
 
@@ -441,8 +458,13 @@ int nvrx_plan_create_at(int64_t n, const void* const* ptrs, const uint64_t* nbyt
 
 int nvrx_plan_destroy(nvrx_plan* p) {
     if (!p) return NVRX_OK;
-    if (p->pin_segs || p->pin_tiles || p->d_segs || p->d_tiles || !p->chunk_events.empty() || p->upload_done) {
+    if (p->pin_segs || p->pin_tiles || p->d_segs || p->d_tiles || !p->chunk_events.empty() || p->upload_done ||
+        p->last_launch) {
         DeviceGuard guard(p->device);
+        if (p->last_launch) {
+            cudaEventSynchronize(p->last_launch);  // a queued launch may still read the mirrors freed below
+            cudaEventDestroy(p->last_launch);
+        }
         if (p->upload_done) cudaEventDestroy(p->upload_done);
         if (p->pin_segs) cudaFreeHost(p->pin_segs);
         if (p->pin_tiles) cudaFreeHost(p->pin_tiles);

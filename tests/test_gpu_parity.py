@@ -107,8 +107,9 @@ def test_scatter_roundtrip_into_other_alignments(built_library, variant, tile):
     plan.close()
 
 
+@pytest.mark.parametrize("variant", ["ldg", "tma"])  # tma: narrowed tiles run on the walker's 3 ragged warps
 @pytest.mark.parametrize("tile", [4096, 65536])
-def test_narrow_pack_and_widen_scatter(built_library, tile):
+def test_narrow_pack_and_widen_scatter(built_library, variant, tile):
     g = torch.Generator(device="cuda").manual_seed(4)
     base = torch.randn(900_000, device="cuda", generator=g) * 0.02
     edge = torch.tensor([float("inf"), float("-inf"), float("nan"), -0.0, 0.0, 1e-40, -1e-45, 3.3895314e38, -3.4e38, 1.0, 1.00390625,
@@ -118,7 +119,7 @@ def test_narrow_pack_and_widen_scatter(built_library, tile):
     sq = torch.rand(300_000, device="cuda", generator=g) * 1e-38  # denormal-range magnitudes (Adam exp_avg_sq like)
     tensors = [base[:300_001], base[300_001 + 1 : 300_001 + 1 + 8193], base[400_003:400_003 + 77], sq, torch.tensor(3.0, device="cuda"),
                torch.randint(0, 9, (100,), device="cuda", generator=g), torch.empty(0, device="cuda")]
-    plan = _plan(tensors, narrow=True, tile_bytes=tile)
+    plan = _plan(tensors, narrow=True, tile_bytes=tile, variant=VARIANTS[variant])
     exp, offs, packed = orc.pack_oracle(tensors, narrow=True)
     assert list(plan.offsets) == offs and list(plan.packed_nbytes) == packed
     assert plan.algorithmic_bytes == sum(t.numel() * t.element_size() for t in tensors) + sum(packed)

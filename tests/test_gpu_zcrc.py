@@ -15,7 +15,17 @@ from oracle import crc_oracle as co
 pytestmark = pytest.mark.gpu  # part of the default suite
 
 
-def test_kernel_values_match_zlib(built_library):
+def test_kernel_values_match_zlib(built_library, monkeypatch):
+    monkeypatch.delenv("NVRX_B200_CRC_VARIANT", raising=False)  # crc_chunks_private<32>, the default kernel
+    _check_kernel_values_match_zlib()
+
+
+def test_shared_kernel_values_match_zlib(built_library, monkeypatch):
+    monkeypatch.setenv("NVRX_B200_CRC_VARIANT", "shared")  # crc_chunks<8>: one copy of the tables per CTA, read at every launch
+    _check_kernel_values_match_zlib()
+
+
+def _check_kernel_values_match_zlib():
     from nvidia_resiliency_ext.checkpointing.b200.engine import CrcPlan, finish_crcs
 
     g = torch.Generator(device="cuda").manual_seed(9)
