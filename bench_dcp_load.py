@@ -8,7 +8,11 @@ state (bench.py's workload), stock ``FileSystemReader`` against ``CachedMetadata
 Prints one JSON line.  Per layout and arm: wall time to device sync and GB/s; for the engine arm the box-kernel time (CUDA
 events around the launches only), its
 algorithmic bytes and their share of 3.35 TB/s, the peak staging bytes; and whether every loaded tensor is bit-equal
-between the arms.  Checkpoints go to a temporary directory (``/dev/shm`` when writable) and are removed after each layout."""
+between the arms.  Checkpoints go to a temporary directory (``/dev/shm`` when writable) and are removed after each layout.
+
+``--saved-dtype`` / ``--target-dtype`` (fp32, bf16, fp16; default ``same``) save the floating tensors of the state in one
+dtype and load them into targets of another, so the engine arm converts in the box scatter (algorithmic bytes
+(es + ed) x elements) and bit-equality is NaN-aware (NaN positions by isnan, everything else by bits)."""
 import argparse
 import json
 import os
@@ -28,6 +32,14 @@ import torch  # noqa: E402
 import torch.distributed.checkpoint as dcp  # noqa: E402
 
 HBM_GBS = 3350.0  # H100 SXM data sheet
+DTYPES = {"fp32": torch.float32, "bf16": torch.bfloat16, "fp16": torch.float16}
+
+
+def _as(dtype_name, t):
+    """``t`` in dtype ``dtype_name`` when it is an fp32 / bf16 / fp16 tensor and the name is not ``same``."""
+    if dtype_name == "same" or t.dtype not in DTYPES.values():
+        return t
+    return t.to(DTYPES[dtype_name])
 
 
 def _flat_state(device, scale):
@@ -37,7 +49,7 @@ def _flat_state(device, scale):
     return {f"t{i:04d}": t for i, t in enumerate(flatten(sd))}
 
 
-def _save_sharded(rank, world, port, root, placement, scale):
+def _save_sharded(rank, world, port, root, placement, scale, saved_dtype="same"):
     import torch.distributed as dist
     from torch.distributed.device_mesh import init_device_mesh
     from torch.distributed.tensor import Replicate, Shard, distribute_tensor
@@ -47,6 +59,7 @@ def _save_sharded(rank, world, port, root, placement, scale):
     mesh = init_device_mesh("cpu", (world,))
     sd = {}
     for k, v in _flat_state("cpu", scale).items():
+        v = _as(saved_dtype, v)
         pl = Shard(placement) if v.dim() > placement else (Shard(0) if v.dim() else Replicate())
         sd[k] = distribute_tensor(v, mesh, [pl])
     dcp.save(sd, checkpoint_id=root)
@@ -69,6 +82,13 @@ def _bits_equal(a, b):
         a.numel() == 0 or torch.equal(a.contiguous().view(-1).view(torch.uint8), b.contiguous().view(-1).view(torch.uint8)))
 
 
+def _nan_aware_equal(a, b):
+    if a.dtype not in DTYPES.values() or a.dtype != b.dtype or a.shape != b.shape:
+        return _bits_equal(a, b)
+    na, nb = torch.isnan(a), torch.isnan(b)
+    return torch.equal(na, nb) and _bits_equal(torch.where(na, torch.zeros_like(a), a), torch.where(nb, torch.zeros_like(b), b))
+
+
 def run(args):
     from nvidia_resiliency_ext.checkpointing.async_ckpt.cached_metadata_filesystem_reader import CachedMetadataFileSystemReader
     from nvidia_resiliency_ext.checkpointing.b200.engine import SnapshotEngine
@@ -79,8 +99,10 @@ def run(args):
     torch.cuda.set_device(local)
 
     base = "/dev/shm" if os.access("/dev/shm", os.W_OK) else None
-    like = _flat_state("cuda", args.scale)
+    like = {k: _as(args.saved_dtype, v) for k, v in _flat_state("cuda", args.scale).items()}
     total = sum(t.nbytes for t in like.values())
+    cast = args.saved_dtype != "same" or args.target_dtype != "same"
+    equal = _nan_aware_equal if cast else _bits_equal
     engine = SnapshotEngine.get(local)
     engine.timing = True  # box-kernel time from CUDA events around every launch
     card, power = _card()
@@ -93,13 +115,14 @@ def run(args):
             else:
                 ctx = mp.get_context("spawn")
                 port = 29600 + (os.getpid() % 200)
-                procs = [ctx.Process(target=_save_sharded, args=(r, 2, port, root, int(layout[-1]), args.scale)) for r in range(2)]
+                procs = [ctx.Process(target=_save_sharded, args=(r, 2, port, root, int(layout[-1]), args.scale, args.saved_dtype))
+                         for r in range(2)]
                 for p in procs:
                     p.start()
                 for p in procs:
                     p.join()
                 assert all(p.exitcode == 0 for p in procs), [p.exitcode for p in procs]
-            outs = {arm: {k: torch.empty_like(v) for k, v in like.items()} for arm in ("stock", "engine")}
+            outs = {arm: {k: torch.empty_like(_as(args.target_dtype, v)) for k, v in like.items()} for arm in ("stock", "engine")}
             times = {"stock": [], "engine": []}
             box_ms, stats = [], None
             for it in range(args.warmup + args.steps):
@@ -129,17 +152,20 @@ def run(args):
                 "box_share_of_3p35TBps": round(stats["algorithmic_bytes"] / (kms * 1e-3) / (HBM_GBS * 1e9), 4) if kms else None,
                 "box_batches": stats["batches"],
                 "peak_staging_bytes": stats["peak_staging_bytes"],
-                "bits_equal": all(_bits_equal(outs["stock"][k], outs["engine"][k]) for k in like),
+                "bits_equal": all(equal(outs["stock"][k], outs["engine"][k]) for k in like),
             }
             del outs
         finally:
             shutil.rmtree(root, ignore_errors=True)
+    config = {"workload": f"C2 state ({total / 1e9:.2f} GB, scale {args.scale}) through dcp.save / dcp.load",
+              "steps": args.steps, "warmup": args.warmup, "staging_budget_bytes": SnapshotEngine.DCP_LOAD_STAGING}
+    if cast:
+        config.update(saved_dtype=args.saved_dtype, target_dtype=args.target_dtype)
     return {
         "metric": "dcp_load_GBps",
         "value": layouts["same"]["engine_GBps"],
         "unit": "GB/s",
-        "config": {"workload": f"C2 state ({total / 1e9:.2f} GB, scale {args.scale}) through dcp.save / dcp.load",
-                   "steps": args.steps, "warmup": args.warmup, "staging_budget_bytes": SnapshotEngine.DCP_LOAD_STAGING},
+        "config": config,
         "gpu": card,
         "power_limit": power,
         "layouts": layouts,
@@ -153,6 +179,8 @@ def main():
     ap.add_argument("--steps", type=int, default=3, help="timed loads per layout and arm")
     ap.add_argument("--warmup", type=int, default=1)
     ap.add_argument("--scale", type=float, default=1.0, help="shrink the state (numbers at != 1.0 are not C2)")
+    ap.add_argument("--saved-dtype", choices=["same", *DTYPES], default="same", help="dtype the float tensors are saved in")
+    ap.add_argument("--target-dtype", choices=["same", *DTYPES], default="same", help="dtype of the float targets")
     args = ap.parse_args()
     if args.gpus != 1:
         ap.error("dcp-load runs on one GPU (--gpus 1)")

@@ -34,7 +34,7 @@
 extern "C" {
 #endif
 
-#define NVRX_ABI_VERSION 3
+#define NVRX_ABI_VERSION 4
 
 enum {
     NVRX_OK = 0,
@@ -182,7 +182,7 @@ int nvrx_fill_from_fd(void* staging, uint64_t staging_bytes, int fd, int64_t n, 
  * The planner drops size-1 dims, merges dims that are contiguous on both sides and, when the innermost dim is contiguous
  * on both sides, copies whole "runs" with the vector copy of nvrx_scatter; otherwise it moves one element per thread.  A
  * tile is (box, first row, rows, byte range): descriptors grow with boxes + tiles, not with rows.  No CUDA call is made
- * by create / info / tiles / box. */
+ * by create / create_cast / info / tiles / box / box_cast. */
 #define NVRX_BOX_MAXDIM 8
 typedef struct nvrx_boxplan nvrx_boxplan;
 int nvrx_boxplan_create(int64_t n, const uint32_t* elem_bytes, const int32_t* ndim, const int64_t* sizes,
@@ -190,21 +190,47 @@ int nvrx_boxplan_create(int64_t n, const uint32_t* elem_bytes, const int32_t* nd
                         const int64_t* dst_strides, uint64_t staging_bytes, uint32_t tile_bytes, int device,
                         nvrx_boxplan** out);
 int nvrx_boxplan_destroy(nvrx_boxplan* plan);
-/* tiles of one launch / algorithmic HBM bytes of it (2 x the bytes moved) */
+/* nvrx_boxplan_create, converting between fp32, bf16 and fp16 on the way (loading a checkpoint into a model of another dtype).  cast[i] is
+ * one NVRX_CAST_* code per box (cast == NULL or cast[i] == 0: bit copy, exactly as nvrx_boxplan_create plans it).  For a
+ * converting box elem_bytes[i] is the SOURCE element size and must match the code, src_offs[i] (bytes) must be a multiple
+ * of it and dst_ptrs[i] a multiple of the destination element size; src_strides count source elements, dst_strides
+ * destination elements.  Otherwise NVRX_E_INVALID (as for an unknown code).  Narrowing rounds to nearest even, keeps
+ * subnormals, sends overflow to +-inf and writes NaN as 0x7FFF; widening is exact (bf16 <-> fp16 goes through fp32).  The
+ * converting boxes' tiles follow all copy tiles. */
+#define NVRX_CAST_NONE 0u
+#define NVRX_CAST_F32_BF16 1u
+#define NVRX_CAST_F32_F16 2u
+#define NVRX_CAST_BF16_F32 3u
+#define NVRX_CAST_F16_F32 4u
+#define NVRX_CAST_BF16_F16 5u
+#define NVRX_CAST_F16_BF16 6u
+int nvrx_boxplan_create_cast(int64_t n, const uint32_t* elem_bytes, const int32_t* ndim, const int64_t* sizes,
+                             const uint64_t* src_offs, const int64_t* src_strides, const void* const* dst_ptrs,
+                             const int64_t* dst_strides, const uint32_t* cast, uint64_t staging_bytes, uint32_t tile_bytes,
+                             int device, nvrx_boxplan** out);
+/* tiles of one nvrx_box_scatter / algorithmic HBM bytes of it: (es + ed) x numel per box, es / ed the source / destination
+ * element sizes (2 x the bytes moved for a bit copy) */
 int nvrx_boxplan_info(const nvrx_boxplan* plan, uint64_t* n_tiles, uint64_t* algorithmic_bytes);
 /* Introspection (tests, tooling), like nvrx_plan_tiles: tile t covers rows [row[t], row[t] + nrows[t]) of box box[t]; with
  * one row it covers bytes [byte_off[t], byte_off[t] + nbytes[t]) of it, with several the whole rows.  Up to `capacity`
- * entries are written (any array may be NULL). */
+ * entries are written (any array may be NULL).  For a converting box byte_off / nbytes (and row_bytes below) count SOURCE
+ * bytes, multiples of es; the destination bytes are byte_off / es * ed and nbytes / es * ed. */
 int nvrx_boxplan_tiles(const nvrx_boxplan* plan, uint64_t* n_tiles, uint32_t* box, uint64_t* row, uint64_t* nrows,
                        uint64_t* byte_off, uint32_t* nbytes, uint64_t capacity);
 /* The row geometry the planner made of box i: row r (mixed radix over sizes[0..n_outer), outermost first) is the
  * row_bytes bytes at staging offset src_off + sum idx_d * src_stride[d] and at device address dst + sum idx_d * dst_stride[d]
- * (byte strides).  Arrays hold NVRX_BOX_MAXDIM entries. */
+ * (byte strides; for a converting box row_bytes and src_stride in source bytes, dst_stride in destination bytes).  Arrays
+ * hold NVRX_BOX_MAXDIM entries. */
 int nvrx_boxplan_box(const nvrx_boxplan* plan, int64_t i, uint64_t* row_bytes, uint32_t* n_outer, uint64_t* sizes,
                      int64_t* src_stride, int64_t* dst_stride, uint64_t* src_off, uint64_t* dst);
+/* The NVRX_CAST_* code of box i and its destination element size (the source size for a bit copy); either may be NULL. */
+int nvrx_boxplan_box_cast(const nvrx_boxplan* plan, int64_t i, uint32_t* cast, uint32_t* dst_elem_bytes);
 /* Upload the descriptor tables on `stream` (otherwise done by the first nvrx_box_scatter), e.g. to time the kernel alone. */
 int nvrx_boxplan_commit(nvrx_boxplan* plan, void* stream);
-/* staging -> destination views, ONE kernel launch on `stream` (grid sized from the SM count). */
+/* staging -> destination views on `stream` (grids sized from the SM count): ONE kernel launch over the copy tiles, then
+ * one over the converting tiles; a plan without converting boxes makes exactly one launch.  With converting boxes
+ * `staging` must be 4-byte aligned; the vector body of a converting run needs the staging and destination addresses of
+ * an element to sit at the same position in their vectors (see DESIGN.md), anything else runs element by element. */
 int nvrx_box_scatter(nvrx_boxplan* plan, const void* staging, void* stream);
 
 /* ---- device staging / stream helpers (so callers need no CUDA binding of their own) ---------- */

@@ -27,7 +27,9 @@ struct nvrx_boxplan {
     int sm_count = 0;
     uint64_t algo_bytes = 0;
     std::vector<BoxDesc> boxes;  // host copies are authoritative; the device mirrors are made by commit / the first launch
-    std::vector<BoxTile> tiles;
+    std::vector<BoxTile> tiles;  // [0, n_copy_tiles): bit copies (walk_box); the rest convert (walk_box_cast)
+    size_t n_copy_tiles = 0;
+    std::vector<uint32_t> dst_elem;  // destination element size of each box (introspection only)
     BoxDesc* d_boxes = nullptr;
     BoxTile* d_tiles = nullptr;
     bool uploaded = false;
@@ -50,11 +52,20 @@ struct DeviceGuard {
     }
 };
 
-// One box -> its canonical row geometry (BoxDesc) and the bytes it moves; NVRX_E_INVALID on malformed input.
-int canonical_box(uint32_t elem, int32_t nd, const int64_t* sizes, uint64_t src_off, const int64_t* sst, const void* dst,
-                  const int64_t* dstr, uint64_t staging_bytes, BoxDesc* out, uint64_t* moved) {
+// element sizes (source, destination) of each cast code; index 0 (bit copy) takes the box's own size
+constexpr uint32_t kCastElem[nvrx::kCastCount][2] = {{0, 0}, {4, 2}, {4, 2}, {2, 4}, {2, 4}, {2, 2}, {2, 2}};
+static_assert(NVRX_CAST_F32_BF16 == nvrx::kCastF32Bf16 && NVRX_CAST_F32_F16 == nvrx::kCastF32F16 &&
+                  NVRX_CAST_BF16_F32 == nvrx::kCastBf16F32 && NVRX_CAST_F16_F32 == nvrx::kCastF16F32 &&
+                  NVRX_CAST_BF16_F16 == nvrx::kCastBf16F16 && NVRX_CAST_F16_BF16 == nvrx::kCastF16Bf16,
+              "header and kernel disagree on the cast codes");
+
+// One box -> its canonical row geometry (BoxDesc) and its element count; NVRX_E_INVALID on malformed input.  es / ed are
+// the source / destination element sizes (equal for a bit copy): source offsets, row_bytes and source strides come out in
+// source bytes, destination strides in destination bytes.
+int canonical_box(uint32_t es, uint32_t ed, int32_t nd, const int64_t* sizes, uint64_t src_off, const int64_t* sst,
+                  const void* dst, const int64_t* dstr, uint64_t staging_bytes, BoxDesc* out, uint64_t* numel_out) {
     if (nd < 0 || nd > NVRX_BOX_MAXDIM) return NVRX_E_INVALID;
-    if (!(elem == 1 || elem == 2 || elem == 4 || elem == 8 || elem == 16)) return NVRX_E_INVALID;
+    if (!(es == 1 || es == 2 || es == 4 || es == 8 || es == 16)) return NVRX_E_INVALID;
     uint64_t numel = 1;
     for (int k = 0; k < nd; ++k) {
         if (sizes[k] < 0 || sst[k] < 0 || dstr[k] < 0) return NVRX_E_INVALID;
@@ -62,12 +73,12 @@ int canonical_box(uint32_t elem, int32_t nd, const int64_t* sizes, uint64_t src_
         numel *= static_cast<uint64_t>(sizes[k]);
     }
     memset(out, 0, sizeof(*out));
-    *moved = 0;
+    *numel_out = 0;
     if (numel == 0) return NVRX_OK;  // empty box: no tiles (row_bytes stays 0)
     if (!dst) return NVRX_E_INVALID;
     // last source byte (all strides >= 0: the element at the far corner)
-    uint64_t last = src_off + elem;
-    for (int k = 0; k < nd; ++k) last += static_cast<uint64_t>(sizes[k] - 1) * static_cast<uint64_t>(sst[k]) * elem;
+    uint64_t last = src_off + es;
+    for (int k = 0; k < nd; ++k) last += static_cast<uint64_t>(sizes[k] - 1) * static_cast<uint64_t>(sst[k]) * es;
     if (last > staging_bytes || last < src_off) return NVRX_E_INVALID;
     // drop size-1 dims, then merge neighbours that are contiguous on both sides
     uint64_t sz[NVRX_BOX_MAXDIM];
@@ -90,24 +101,26 @@ int canonical_box(uint32_t elem, int32_t nd, const int64_t* sizes, uint64_t src_
     out->src = src_off;
     out->dst = reinterpret_cast<uint64_t>(dst);
     if (m > 0 && ss[m - 1] == 1 && ds[m - 1] == 1) {
-        out->row_bytes = sz[m - 1] * elem;  // a run: the innermost dim is contiguous on both sides
+        out->row_bytes = sz[m - 1] * es;  // a run: the innermost dim is contiguous on both sides
         --m;
     } else {
-        out->row_bytes = elem;  // element-wise
+        out->row_bytes = es;  // element-wise
     }
     out->n_outer = static_cast<uint32_t>(m);
     for (int k = 0; k < m; ++k) {
         out->size[k] = sz[k];
-        out->sstr[k] = ss[k] * static_cast<int64_t>(elem);
-        out->dstr[k] = ds[k] * static_cast<int64_t>(elem);
+        out->sstr[k] = ss[k] * static_cast<int64_t>(es);
+        out->dstr[k] = ds[k] * static_cast<int64_t>(ed);
     }
-    *moved = numel * elem;
+    *numel_out = numel;
     return NVRX_OK;
 }
 
-// Tiles of ~tile_bytes: a row longer than half a tile is cut into byte ranges, shorter rows are grouped.
-void box_tiles(const BoxDesc& b, uint32_t index, uint32_t tile_bytes, std::vector<BoxTile>& tiles) {
+// Tiles of ~tile_bytes on the wider side (source bytes tile_bytes / max(es, ed) * es, a multiple of es; tile_bytes itself
+// for a bit copy): a row longer than half a tile is cut into byte ranges, shorter rows are grouped.
+void box_tiles(const BoxDesc& b, uint32_t index, uint32_t tile_bytes, uint32_t es, uint32_t ed, std::vector<BoxTile>& tiles) {
     if (b.row_bytes == 0) return;
+    tile_bytes = tile_bytes / std::max(es, ed) * es;
     uint64_t rows = 1;
     for (uint32_t k = 0; k < b.n_outer; ++k) rows *= b.size[k];
     BoxTile t;
@@ -134,14 +147,9 @@ void box_tiles(const BoxDesc& b, uint32_t index, uint32_t tile_bytes, std::vecto
     }
 }
 
-}  // namespace
-
-extern "C" {
-
-int nvrx_boxplan_create(int64_t n, const uint32_t* elem_bytes, const int32_t* ndim, const int64_t* sizes,
-                        const uint64_t* src_offs, const int64_t* src_strides, const void* const* dst_ptrs,
-                        const int64_t* dst_strides, uint64_t staging_bytes, uint32_t tile_bytes, int device,
-                        nvrx_boxplan** out) {
+int boxplan_create(int64_t n, const uint32_t* elem_bytes, const int32_t* ndim, const int64_t* sizes, const uint64_t* src_offs,
+                   const int64_t* src_strides, const void* const* dst_ptrs, const int64_t* dst_strides, const uint32_t* cast,
+                   uint64_t staging_bytes, uint32_t tile_bytes, int device, nvrx_boxplan** out) {
     if (!out || n < 0 || (n > 0 && (!elem_bytes || !ndim || !src_offs || !dst_ptrs))) return NVRX_E_INVALID;
     if (n > 0xffffffffll) return NVRX_E_INVALID;
     if (tile_bytes == 0) tile_bytes = kDefaultBoxTile;
@@ -157,19 +165,36 @@ int nvrx_boxplan_create(int64_t n, const uint32_t* elem_bytes, const int32_t* nd
     try {  // the ABI never throws: container growth failures become NVRX_E_NOMEM
         p->device = device;
         p->boxes.resize(static_cast<size_t>(n));
+        p->dst_elem.resize(static_cast<size_t>(n));
+        std::vector<BoxTile> cast_tiles;
         int64_t d0 = 0;
         for (int64_t i = 0; i < n; ++i) {
-            uint64_t moved = 0;
-            int rc = canonical_box(elem_bytes[i], ndim[i], sizes + d0, src_offs[i], src_strides + d0, dst_ptrs[i],
-                                   dst_strides + d0, staging_bytes, &p->boxes[i], &moved);
+            const uint32_t code = cast ? cast[i] : 0u;
+            uint32_t es = elem_bytes[i], ed = es;
+            int rc = NVRX_OK;
+            if (code >= nvrx::kCastCount) {
+                rc = NVRX_E_INVALID;
+            } else if (code != 0) {
+                ed = kCastElem[code][1];
+                if (es != kCastElem[code][0] || src_offs[i] % es != 0 || reinterpret_cast<uintptr_t>(dst_ptrs[i]) % ed != 0)
+                    rc = NVRX_E_INVALID;
+            }
+            uint64_t numel = 0;
+            if (rc == NVRX_OK)
+                rc = canonical_box(es, ed, ndim[i], sizes + d0, src_offs[i], src_strides + d0, dst_ptrs[i], dst_strides + d0,
+                                   staging_bytes, &p->boxes[i], &numel);
             if (rc) {
                 delete p;
                 return rc;
             }
-            p->algo_bytes += 2 * moved;
+            p->boxes[i].cast = code;
+            p->dst_elem[i] = ed;
+            p->algo_bytes += numel * (es + ed);
             d0 += ndim[i];
-            box_tiles(p->boxes[i], static_cast<uint32_t>(i), tile_bytes, p->tiles);
+            box_tiles(p->boxes[i], static_cast<uint32_t>(i), tile_bytes, es, ed, code ? cast_tiles : p->tiles);
         }
+        p->n_copy_tiles = p->tiles.size();
+        p->tiles.insert(p->tiles.end(), cast_tiles.begin(), cast_tiles.end());
         if (p->tiles.size() > 0xffffffffull) {
             delete p;
             return NVRX_E_INVALID;
@@ -180,6 +205,26 @@ int nvrx_boxplan_create(int64_t n, const uint32_t* elem_bytes, const int32_t* nd
     }
     *out = p;
     return NVRX_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int nvrx_boxplan_create(int64_t n, const uint32_t* elem_bytes, const int32_t* ndim, const int64_t* sizes,
+                        const uint64_t* src_offs, const int64_t* src_strides, const void* const* dst_ptrs,
+                        const int64_t* dst_strides, uint64_t staging_bytes, uint32_t tile_bytes, int device,
+                        nvrx_boxplan** out) {
+    return boxplan_create(n, elem_bytes, ndim, sizes, src_offs, src_strides, dst_ptrs, dst_strides, nullptr, staging_bytes,
+                          tile_bytes, device, out);
+}
+
+int nvrx_boxplan_create_cast(int64_t n, const uint32_t* elem_bytes, const int32_t* ndim, const int64_t* sizes,
+                             const uint64_t* src_offs, const int64_t* src_strides, const void* const* dst_ptrs,
+                             const int64_t* dst_strides, const uint32_t* cast, uint64_t staging_bytes, uint32_t tile_bytes,
+                             int device, nvrx_boxplan** out) {
+    return boxplan_create(n, elem_bytes, ndim, sizes, src_offs, src_strides, dst_ptrs, dst_strides, cast, staging_bytes,
+                          tile_bytes, device, out);
 }
 
 int nvrx_boxplan_destroy(nvrx_boxplan* p) {
@@ -231,6 +276,14 @@ int nvrx_boxplan_box(const nvrx_boxplan* p, int64_t i, uint64_t* row_bytes, uint
     return NVRX_OK;
 }
 
+int nvrx_boxplan_box_cast(const nvrx_boxplan* p, int64_t i, uint32_t* cast, uint32_t* dst_elem_bytes) {
+    if (!p || i < 0 || static_cast<uint64_t>(i) >= p->boxes.size()) return NVRX_E_INVALID;
+    const BoxDesc& b = p->boxes[static_cast<size_t>(i)];
+    if (cast) *cast = b.cast;
+    if (dst_elem_bytes) *dst_elem_bytes = p->dst_elem[static_cast<size_t>(i)];
+    return NVRX_OK;
+}
+
 namespace {
 
 int box_upload(nvrx_boxplan* p, cudaStream_t st) {
@@ -259,16 +312,25 @@ int nvrx_box_scatter(nvrx_boxplan* p, const void* staging, void* stream) {
     if (!p) return NVRX_E_INVALID;
     if (p->tiles.empty()) return NVRX_OK;
     if (!staging) return NVRX_E_INVALID;
+    const uint32_t ncopy = static_cast<uint32_t>(p->n_copy_tiles);
+    const uint32_t ncast = static_cast<uint32_t>(p->tiles.size() - p->n_copy_tiles);
+    if (ncast && reinterpret_cast<uintptr_t>(staging) % 4 != 0) return NVRX_E_INVALID;  // source elements must be aligned
     DeviceGuard guard(p->device);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     int rc = box_upload(p, st);
     if (rc) return rc;
-    const uint32_t ntiles = static_cast<uint32_t>(p->tiles.size());
-    uint32_t grid = static_cast<uint32_t>(p->sm_count) * 8;  // 8 resident CTAs of 256 threads per SM
-    grid = std::max<uint32_t>(1, std::min(grid, ntiles));
-    nvrx::walk_box<<<grid, nvrx::kBoxThreads, 0, st>>>(p->d_boxes, p->d_tiles, ntiles,
-                                                       const_cast<uint8_t*>(static_cast<const uint8_t*>(staging)));
-    NVRX_CUDA(cudaGetLastError());
+    uint8_t* stg = const_cast<uint8_t*>(static_cast<const uint8_t*>(staging));
+    const uint32_t max_grid = static_cast<uint32_t>(p->sm_count) * 8;  // 8 resident CTAs of 256 threads per SM
+    if (ncopy) {
+        const uint32_t grid = std::max<uint32_t>(1, std::min(max_grid, ncopy));
+        nvrx::walk_box<<<grid, nvrx::kBoxThreads, 0, st>>>(p->d_boxes, p->d_tiles, ncopy, stg);
+        NVRX_CUDA(cudaGetLastError());
+    }
+    if (ncast) {
+        const uint32_t grid = std::max<uint32_t>(1, std::min(max_grid, ncast));
+        nvrx::walk_box_cast<<<grid, nvrx::kBoxThreads, 0, st>>>(p->d_boxes, p->d_tiles + ncopy, ncast, stg);
+        NVRX_CUDA(cudaGetLastError());
+    }
     return NVRX_OK;
 }
 

@@ -7,7 +7,10 @@ global metadata only the first time.  The cache is per class, keyed by the absol
 ``load_on_engine=True`` (opt-in) loads the tensor items whose targets are CUDA tensors of this device through the H100
 snapshot engine instead of ``FileSystemReader.read_data``'s per-item ``torch.load`` + ``narrow`` + pageable ``copy_``: only
 the byte span each read item needs goes file -> pinned ring -> HBM, and one box-scatter kernel per staging batch writes
-every (possibly resharded, possibly non-contiguous) target view.  See ``SnapshotEngine.load_boxes``."""
+every (possibly resharded, possibly non-contiguous) target view.  Items saved as fp32, bf16 or fp16 and loaded into a
+target of another of the three dtypes (an fp32 checkpoint into a bf16 model, bf16 weights into fp32 master parameters) are
+converted by that kernel, rounding to nearest even like ``Tensor.to``; bits match the stock reader except for NaN payloads.
+See ``SnapshotEngine.load_boxes``."""
 
 import dataclasses
 import os
@@ -18,15 +21,18 @@ from torch.distributed.checkpoint import FileSystemReader, Metadata
 from torch.distributed.checkpoint.planner import LoadItemType, LoadPlan, LoadPlanner
 from torch.futures import Future
 
+# dtypes the engine converts between on the device (any other dtype mismatch takes FileSystemReader's path)
+_DEVICE_CAST_DTYPES = (torch.float32, torch.bfloat16, torch.float16)
+
 
 class CachedMetadataFileSystemReader(FileSystemReader):
     _metadata_cache: Dict[str, Metadata] = {}
 
     def __init__(self, path: Union[str, os.PathLike], cache_metadata: bool = True, *, load_on_engine: bool = False) -> None:
         """``cache_metadata=False`` makes this a plain ``FileSystemReader`` (every ``read_metadata`` hits the disk).
-        ``load_on_engine=True``: tensor items bound for CUDA tensors of the current device, stored with their target's dtype
-        and without storage transforms, are loaded by the snapshot engine; everything else takes ``FileSystemReader``'s
-        path.  Raises like ``SnapshotEngine`` when there is no CUDA device or no engine library (no silent fallback)."""
+        ``load_on_engine=True``: tensor items bound for CUDA tensors of the current device, stored without storage
+        transforms and with their target's dtype (or fp32 / bf16 / fp16 into another of these three, converted on the
+        device), are loaded by the snapshot engine; everything else takes ``FileSystemReader``'s path.  Raises like ``SnapshotEngine`` when there is no CUDA device or no engine library (no silent fallback)."""
         super().__init__(path=path)
         self._cache_key: Optional[str] = os.path.abspath(os.fspath(path)) if cache_metadata else None
         self._load_on_engine = bool(load_on_engine)
@@ -65,33 +71,37 @@ class CachedMetadataFileSystemReader(FileSystemReader):
             saved = saved_md.get(req.storage_index.fqn)
             if req.type == LoadItemType.TENSOR and not getattr(info, "transform_descriptors", None) and saved is not None:
                 target = planner.resolve_tensor(req).detach()
-                if target.is_cuda and target.get_device() == engine.device and target.dtype == saved.properties.dtype:
-                    mine.append((req, info, target))
+                saved_dtype = saved.properties.dtype
+                same = target.dtype == saved_dtype
+                cast = target.dtype in _DEVICE_CAST_DTYPES and saved_dtype in _DEVICE_CAST_DTYPES
+                if target.is_cuda and target.get_device() == engine.device and (same or cast):
+                    mine.append((req, info, target, saved_dtype))
                     continue
             rest.append(req)
         if mine:
             entries, chunks, fds = [], {}, {}
             try:
-                for req, info, target in mine:
+                for req, info, target, saved_dtype in mine:
                     path = os.fspath(self.fs.concat_path(self.path, info.relative_path))
                     chunk = chunks.get((path, info.offset))
                     if chunk is None:
                         if path not in fds:
                             fds[path] = os.open(path, os.O_RDONLY)
                         chunk = chunks[(path, info.offset)] = read_tensor_record(fds[path], info.offset, info.length)
-                    if chunk.dtype != target.dtype:
-                        raise ValueError(f"{req.storage_index.fqn}: stored as {chunk.dtype}, metadata says {target.dtype}")
+                    if chunk.dtype != saved_dtype:
+                        raise ValueError(f"{req.storage_index.fqn}: stored as {chunk.dtype}, metadata says {saved_dtype}")
                     if tuple(target.shape) != tuple(req.lengths):
                         raise AssertionError(f"req {req.storage_index} mismatch sizes {tuple(target.shape)} vs {tuple(req.lengths)}")
                     src_offset = chunk.storage_offset + sum(o * s for o, s in zip(req.storage_offsets, chunk.stride))
                     entries.append(
-                        BoxLoad(path, chunk.data_off, chunk.numel * target.element_size(), src_offset, chunk.stride, target)
+                        BoxLoad(path, chunk.data_off, chunk.numel * chunk.dtype.itemsize, src_offset, chunk.stride, target,
+                                None if chunk.dtype == target.dtype else chunk.dtype)
                     )
             finally:
                 for fd in fds.values():
                     os.close(fd)
             engine.load_boxes(entries)  # returns after the device work is done
-            for req, _, target in mine:
+            for req, _, target, _ in mine:
                 planner.commit_tensor(req, target)
         if rest:
             return super().read_data(dataclasses.replace(plan, items=rest), planner)

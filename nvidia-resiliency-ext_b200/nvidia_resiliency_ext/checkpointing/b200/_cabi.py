@@ -12,7 +12,7 @@ import os
 from pathlib import Path
 from typing import Optional
 
-ABI_VERSION = 3
+ABI_VERSION = 4
 
 OK = 0
 E_INVALID = 1000
@@ -26,6 +26,15 @@ SEG_NARROW_F32_BF16 = 0x1
 VARIANT_AUTO = 0
 VARIANT_LDG = 1
 VARIANT_TMA = 2
+
+# nvrx_boxplan_create_cast conversion codes (0 = bit copy)
+CAST_NONE = 0
+CAST_F32_BF16 = 1
+CAST_F32_F16 = 2
+CAST_BF16_F32 = 3
+CAST_F16_F32 = 4
+CAST_BF16_F16 = 5
+CAST_F16_BF16 = 6
 
 # every symbol include/nvrx_snap.h declares; tests check the built library exports all of them
 EXPORTED_SYMBOLS = (
@@ -52,10 +61,12 @@ EXPORTED_SYMBOLS = (
     "nvrx_fill",
     "nvrx_fill_from_fd",
     "nvrx_boxplan_create",
+    "nvrx_boxplan_create_cast",
     "nvrx_boxplan_destroy",
     "nvrx_boxplan_info",
     "nvrx_boxplan_tiles",
     "nvrx_boxplan_box",
+    "nvrx_boxplan_box_cast",
     "nvrx_boxplan_commit",
     "nvrx_box_scatter",
     "nvrx_dev_alloc",
@@ -153,10 +164,14 @@ def _declare(lib: C.CDLL) -> None:
         "nvrx_boxplan_create": (
             _int, [_i64, P(_u32), P(_i32), P(_i64), P(_u64), P(_i64), P(_vp), P(_i64), _u64, _u32, _int, P(_vp)]
         ),
+        "nvrx_boxplan_create_cast": (
+            _int, [_i64, P(_u32), P(_i32), P(_i64), P(_u64), P(_i64), P(_vp), P(_i64), P(_u32), _u64, _u32, _int, P(_vp)]
+        ),
         "nvrx_boxplan_destroy": (_int, [_vp]),
         "nvrx_boxplan_info": (_int, [_vp, P(_u64), P(_u64)]),
         "nvrx_boxplan_tiles": (_int, [_vp, P(_u64), P(_u32), P(_u64), P(_u64), P(_u64), P(_u32), _u64]),
         "nvrx_boxplan_box": (_int, [_vp, _i64, P(_u64), P(_u32), P(_u64), P(_i64), P(_i64), P(_u64), P(_u64)]),
+        "nvrx_boxplan_box_cast": (_int, [_vp, _i64, P(_u32), P(_u32)]),
         "nvrx_boxplan_commit": (_int, [_vp, _vp]),
         "nvrx_box_scatter": (_int, [_vp, _vp, _vp]),
         "nvrx_dev_alloc": (_int, [_int, _u64, P(_vp)]),

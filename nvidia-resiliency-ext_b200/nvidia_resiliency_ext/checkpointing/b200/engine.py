@@ -278,30 +278,55 @@ class CrcPlan:
             pass
 
 
-class BoxPlan:
-    """N-d sub-boxes of chunks in device staging -> N-d sub-boxes of destination views (``nvrx_boxplan_*``), one launch.
-    ``boxes[i] = (elem_bytes, sizes, staging byte offset of element 0, staging strides, destination address, destination
-    strides)``, strides in elements.  Creating it is CUDA-free."""
+# (saved dtype, target dtype) -> nvrx_boxplan_create_cast code: the conversions the box scatter makes on the way
+BOX_CASTS = {
+    (torch.float32, torch.bfloat16): _cabi.CAST_F32_BF16,
+    (torch.float32, torch.float16): _cabi.CAST_F32_F16,
+    (torch.bfloat16, torch.float32): _cabi.CAST_BF16_F32,
+    (torch.float16, torch.float32): _cabi.CAST_F16_F32,
+    (torch.bfloat16, torch.float16): _cabi.CAST_BF16_F16,
+    (torch.float16, torch.bfloat16): _cabi.CAST_F16_BF16,
+}
 
-    def __init__(self, boxes: Sequence[tuple], staging_bytes: int, *, device: int, tile_bytes: int = 0):
+
+def cast_vector_elems(src_dtype: torch.dtype, dst_dtype: torch.dtype) -> int:
+    """Elements per vector of the converting box scatter: 4 for the pairs with fp32 (16 B <-> 8 B), 8 for bf16 <-> fp16."""
+    return 4 if torch.float32 in (src_dtype, dst_dtype) else 8
+
+
+class BoxPlan:
+    """N-d sub-boxes of chunks in device staging -> N-d sub-boxes of destination views (``nvrx_boxplan_*``), one launch
+    (two when ``casts`` mixes bit copies and conversions).  ``boxes[i] = (elem_bytes, sizes, staging byte offset of element
+    0, staging strides, destination address, destination strides)``, strides in elements.  ``casts[i]``: the box's
+    ``_cabi.CAST_*`` code (then ``elem_bytes`` is the source element size); None or all zero plans exactly as without it.
+    Creating it is CUDA-free."""
+
+    def __init__(self, boxes: Sequence[tuple], staging_bytes: int, *, device: int, tile_bytes: int = 0,
+                 casts: Optional[Sequence[int]] = None):
         self._lib = _cabi.lib()
         self._h = C.c_void_p()
         n = len(boxes)
         dims = [len(b[1]) for b in boxes]
         flat = lambda k: [int(v) for b in boxes for v in b[k]]  # noqa: E731
         i64 = lambda vals: (C.c_int64 * max(len(vals), 1))(*vals)  # noqa: E731
-        check(
-            self._lib.nvrx_boxplan_create(
-                n, _u32_array([b[0] for b in boxes]), (C.c_int32 * max(n, 1))(*dims), i64(flat(1)),
-                _u64_array([b[2] for b in boxes]), i64(flat(3)), _ptr_array([b[4] for b in boxes]), i64(flat(5)),
-                staging_bytes, tile_bytes, device, C.byref(self._h),
-            ),
-            "nvrx_boxplan_create",
+        args = (
+            n, _u32_array([b[0] for b in boxes]), (C.c_int32 * max(n, 1))(*dims), i64(flat(1)),
+            _u64_array([b[2] for b in boxes]), i64(flat(3)), _ptr_array([b[4] for b in boxes]), i64(flat(5)),
         )
+        tail = (staging_bytes, tile_bytes, device, C.byref(self._h))
+        if casts is not None and any(casts):
+            check(self._lib.nvrx_boxplan_create_cast(*args, _u32_array(list(casts)), *tail), "nvrx_boxplan_create_cast")
+        else:
+            check(self._lib.nvrx_boxplan_create(*args, *tail), "nvrx_boxplan_create")
         tiles, algo = C.c_uint64(), C.c_uint64()
         check(self._lib.nvrx_boxplan_info(self._h, C.byref(tiles), C.byref(algo)), "nvrx_boxplan_info")
         self.n_tiles = tiles.value
         self.algorithmic_bytes = algo.value
+        # kernels one scatter launches: walk_box over the copy tiles, walk_box_cast over the converting ones (a box has
+        # tiles iff it is not empty)
+        nonempty = [all(int(s) for s in b[1]) for b in boxes]
+        kinds = {bool(casts[i]) if casts is not None else False for i in range(n) if nonempty[i]}
+        self.launches = len(kinds)
 
     def tiles(self) -> List[Tuple[int, int, int, int, int]]:
         """[(box, row, nrows, byte_off, nbytes), ...] -- the work-list as the kernel walks it (no CUDA involved)."""
@@ -334,7 +359,8 @@ class BoxLoad(NamedTuple):
 
     ``file_off`` / ``file_len``: where the chunk's storage bytes sit in ``path``; ``src_offset`` / ``src_strides``: element
     offset of the sub-box's first element in that storage and the chunk's strides (elements).  The box's sizes are
-    ``target.shape``."""
+    ``target.shape``.  ``src_dtype``: the chunk's dtype when it differs from the target's (fp32 / bf16 / fp16 into another
+    of the three, converted on the device); None means the target's dtype."""
 
     path: str
     file_off: int
@@ -342,6 +368,7 @@ class BoxLoad(NamedTuple):
     src_offset: int
     src_strides: Tuple[int, ...]
     target: torch.Tensor
+    src_dtype: Optional[torch.dtype] = None
 
 
 def box_span(sizes: Sequence[int], strides: Sequence[int], elem: int) -> int:
@@ -366,6 +393,18 @@ def split_box(sizes, src_off, sstr, dst_off, dstr, elem: int, limit: int):
     for i in range(0, n, max(k, 1)):
         sub = sizes[:d] + [min(max(k, 1), n - i)] + sizes[d + 1:]
         yield from split_box(sub, src_off + i * sstr[d], sstr, dst_off + i * dstr[d], dstr, elem, limit)
+
+
+def box_stage_pos(cur: int, dst: int, conv: Optional[Tuple[int, int, int]] = None) -> int:
+    """Staging position of a load piece: the first ``pos >= cur`` that lines its first element up with the target address
+    ``dst``.  A bit copy takes ``pos = dst (mod 16)``.  A conversion ``conv = (es, ed, V)`` takes ``pos = 0 (mod es)`` and
+    ``pos / es = dst / ed (mod V)``: the source and destination of an element sit at the same index in their V-element
+    vectors, so the vector body starts at the first element where the destination is vector-aligned."""
+    if conv is None:
+        return cur + (dst - cur) % 16
+    es, ed, v = conv
+    m = -(-cur // es)
+    return (m + (dst // ed - m) % v) * es
 
 
 def finish_crcs(offsets: Sequence[int], nbytes: Sequence[int], values_ptr: int, n_values: int, host_base: int) -> List[int]:
@@ -1211,46 +1250,55 @@ class SnapshotEngine:
 
     def load_boxes(self, entries: Sequence[BoxLoad]) -> None:
         """Resharded load: write the sub-box of a saved chunk described by every entry into its target view (a CUDA tensor of
-        this device, any strides, the chunk's dtype).  Blocking, like ``restore``.
+        this device, any strides, the chunk's dtype or -- fp32 / bf16 / fp16 into another of the three, ``src_dtype`` --
+        converted on the way).  Blocking, like ``restore``.
 
         Only the byte span of each sub-box is read, by ``nvrx_fill_from_fd`` (file -> pinned ring -> staging, one call per
-        file per batch) to a staging position with the same address mod 16 as the target's first byte, so that same-layout
-        loads are aligned 16-byte copies; one ``nvrx_box_scatter`` per batch writes the views.  Batches hold at most
+        file per batch) to a staging position that lines up with the target's first byte (``box_stage_pos``), so that
+        same-layout loads are aligned vector copies or conversions; one ``nvrx_box_scatter`` per batch writes the views.  Batches hold at most
         ``DCP_LOAD_STAGING`` bytes and reuse one buffer: batch k+1's copies are enqueued on the stream after batch k's
         scatter.  An entry larger than a batch is cut along its outermost dim (down to element ranges of a single run)."""
         import time as _time
 
         budget = max(int(self.DCP_LOAD_STAGING), 4096)
-        # pieces: (path, file offset of the span, span bytes, box tuple without staging offset, target address)
+        # pieces: (path, file offset of the span, span bytes, box tuple without staging offset + cast code + (es, ed, V))
         pieces = []
         for e in entries:
             t = e.target
             if not (t.is_cuda and t.get_device() == self.device):
                 raise ValueError("load_boxes: every target must be a CUDA tensor of the engine's device")
-            elem = t.element_size()
+            ed = t.element_size()
+            src_dtype = t.dtype if e.src_dtype is None else e.src_dtype
+            cast, conv = 0, None
+            if src_dtype != t.dtype:
+                cast = BOX_CASTS.get((src_dtype, t.dtype))
+                if cast is None:
+                    raise ValueError(f"load_boxes: no device conversion from {src_dtype} to {t.dtype}")
+                conv = (src_dtype.itemsize, ed, cast_vector_elems(src_dtype, t.dtype))
+            es = src_dtype.itemsize  # spans, bounds and budgets count source (staging) bytes
             sizes, dstr = list(t.shape), list(t.stride())
             sstr = list(e.src_strides)
             if len(sstr) != len(sizes):
                 raise ValueError(f"load_boxes: {len(sizes)}-d target for a {len(sstr)}-d source box")
-            span = box_span(sizes, sstr, elem)
-            if span and (e.src_offset < 0 or e.src_offset * elem + span > e.file_len):
+            span = box_span(sizes, sstr, es)
+            if span and (e.src_offset < 0 or e.src_offset * es + span > e.file_len):
                 raise ValueError(f"load_boxes: box reaches past the saved chunk in {e.path}")
             if span == 0:
                 continue
-            for sz, so, do in split_box(sizes, e.src_offset, sstr, 0, dstr, elem, budget - 16):
-                dst = t.data_ptr() + do * elem
-                pieces.append((e.path, e.file_off + so * elem, box_span(sz, sstr, elem), (elem, sz, sstr, dst, dstr)))
+            for sz, so, do in split_box(sizes, e.src_offset, sstr, 0, dstr, es, budget - 16):
+                dst = t.data_ptr() + do * ed
+                pieces.append((e.path, e.file_off + so * es, box_span(sz, sstr, es), (es, sz, sstr, dst, dstr, cast, conv)))
         # one nvrx_fill_from_fd per file per batch copies each ring chunk from its file's first to its last byte in it, gaps
         # included: the pieces of a file must occupy one staging range of their own, so they are placed file by file (and in
         # file order, which also keeps the reads sequential)
         pieces.sort(key=lambda pc: (pc[0], pc[1]))
-        # batches: a piece starts at the first position >= the cursor that is congruent to its target address mod 16
+        # batches: a piece starts at the first position >= the cursor that box_stage_pos allows (at most 15 bytes later)
         batches, cur = [[]], 0
         for piece in pieces:
-            pos = cur + (piece[3][3] - cur) % 16
+            pos = box_stage_pos(cur, piece[3][3], piece[3][6])
             if batches[-1] and pos + piece[2] > budget:
                 batches.append([])
-                pos = piece[3][3] % 16
+                pos = box_stage_pos(0, piece[3][3], piece[3][6])
             batches[-1].append((pos,) + piece)
             cur = pos + piece[2]
         batches = [b for b in batches if b]
@@ -1287,6 +1335,7 @@ class SnapshotEngine:
                     )
                 plan = BoxPlan(
                     [(b[0], b[1], pos, b[2], b[3], b[4]) for pos, _, _, _, b in batch], end, device=self.device,
+                    casts=[b[5] for _, _, _, _, b in batch],
                 )
                 plans.append(plan)
                 stats["algorithmic_bytes"] += plan.algorithmic_bytes
@@ -1298,7 +1347,7 @@ class SnapshotEngine:
                 if self.timing:
                     ev[1].record(stream)
                     timers.append(ev)
-                self.launches += 1 if plan.n_tiles else 0
+                self.launches += plan.launches
                 self.box_batches += 1
             done = Event(self.device)
             done.record(stream)
