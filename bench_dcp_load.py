@@ -12,7 +12,14 @@ between the arms.  Checkpoints go to a temporary directory (``/dev/shm`` when wr
 
 ``--saved-dtype`` / ``--target-dtype`` (fp32, bf16, fp16; default ``same``) save the floating tensors of the state in one
 dtype and load them into targets of another, so the engine arm converts in the box scatter (algorithmic bytes
-(es + ed) x elements) and bit-equality is NaN-aware (NaN positions by isnan, everything else by bits)."""
+(es + ed) x elements) and bit-equality is NaN-aware (NaN positions by isnan, everything else by bits).
+
+``--verify`` adds a third arm, the engine reader with ``verify=True`` (every record checked against its CRC-32 on the
+GPU), alternating with the other two.  Per layout it adds the arm's wall time, the CRC kernels' time (CUDA events around
+their launches only), the bytes they summed and their share of 3.35 TB/s (reads only: S bytes, not 2 S), the host time
+of the verify path (range planning, CRC plans and launches, chaining), the per-run wall times of both engine arms, the
+bytes read for the checksum alone and whether the arm's tensors are bit-equal to the stock ones.  Without the flag the JSON is
+unchanged."""
 import argparse
 import json
 import os
@@ -122,13 +129,14 @@ def run(args):
                 for p in procs:
                     p.join()
                 assert all(p.exitcode == 0 for p in procs), [p.exitcode for p in procs]
-            outs = {arm: {k: torch.empty_like(_as(args.target_dtype, v)) for k, v in like.items()} for arm in ("stock", "engine")}
-            times = {"stock": [], "engine": []}
-            box_ms, stats = [], None
+            arms = ("stock", "engine", "verified") if args.verify else ("stock", "engine")
+            outs = {arm: {k: torch.empty_like(_as(args.target_dtype, v)) for k, v in like.items()} for arm in arms}
+            times = {arm: [] for arm in arms}
+            box_ms, stats, crc_ms, verify_host_ms, vstats = [], None, [], [], None
             for it in range(args.warmup + args.steps):
-                for arm in ("stock", "engine"):
+                for arm in arms:
                     reader = (dcp.FileSystemReader(root) if arm == "stock"
-                              else CachedMetadataFileSystemReader(root, load_on_engine=True))
+                              else CachedMetadataFileSystemReader(root, load_on_engine=True, verify=arm == "verified"))
                     torch.cuda.synchronize()
                     t0 = time.perf_counter()
                     dcp.load(outs[arm], storage_reader=reader)
@@ -139,6 +147,10 @@ def run(args):
                         if arm == "engine":
                             stats = dict(engine.last_box_load)
                             box_ms.append(stats["box_ms"])
+                        if arm == "verified":
+                            vstats = dict(engine.last_box_load)
+                            crc_ms.append(vstats["crc_ms"])
+                            verify_host_ms.append(vstats["verify_host_ms"])
             CachedMetadataFileSystemReader.clear_metadata_cache()
             med = {arm: sorted(v)[len(v) // 2] for arm, v in times.items()}
             kms = sorted(box_ms)[len(box_ms) // 2]
@@ -152,8 +164,22 @@ def run(args):
                 "box_share_of_3p35TBps": round(stats["algorithmic_bytes"] / (kms * 1e-3) / (HBM_GBS * 1e9), 4) if kms else None,
                 "box_batches": stats["batches"],
                 "peak_staging_bytes": stats["peak_staging_bytes"],
-                "bits_equal": all(equal(outs["stock"][k], outs["engine"][k]) for k in like),
+                "bits_equal": all(equal(outs["stock"][k], outs[arm][k]) for arm in arms[1:] for k in like),
             }
+            if args.verify:
+                cms = sorted(crc_ms)[len(crc_ms) // 2]
+                layouts[layout].update(
+                    engine_verified_s=round(med["verified"], 4),
+                    engine_s_runs=[round(x, 4) for x in times["engine"]],
+                    engine_verified_s_runs=[round(x, 4) for x in times["verified"]],
+                    verify_host_ms=round(sorted(verify_host_ms)[len(verify_host_ms) // 2], 3),
+                    crc_kernel_ms=round(cms, 3),
+                    crc_bytes=vstats["crc_bytes"],
+                    crc_share_of_3p35TBps=round(vstats["crc_bytes"] / (cms * 1e-3) / (HBM_GBS * 1e9), 4) if cms else None,
+                    verified_records=vstats["verified_records"],
+                    unverified_records=vstats["unverified_records"],
+                    verify_extra_bytes=vstats["verify_extra_bytes"],
+                )
             del outs
         finally:
             shutil.rmtree(root, ignore_errors=True)
@@ -181,6 +207,7 @@ def main():
     ap.add_argument("--scale", type=float, default=1.0, help="shrink the state (numbers at != 1.0 are not C2)")
     ap.add_argument("--saved-dtype", choices=["same", *DTYPES], default="same", help="dtype the float tensors are saved in")
     ap.add_argument("--target-dtype", choices=["same", *DTYPES], default="same", help="dtype of the float targets")
+    ap.add_argument("--verify", action="store_true", help="add the engine reader with verify=True as a third arm")
     args = ap.parse_args()
     if args.gpus != 1:
         ap.error("dcp-load runs on one GPU (--gpus 1)")

@@ -34,7 +34,7 @@
 extern "C" {
 #endif
 
-#define NVRX_ABI_VERSION 4
+#define NVRX_ABI_VERSION 5
 
 enum {
     NVRX_OK = 0,
@@ -327,6 +327,31 @@ int nvrx_crc_finish(int64_t n, const uint64_t* offsets, const uint64_t* nbytes, 
                     const void* host_base, uint32_t* out_crcs);
 /* The 4x256-word operator table "feed `which` zero bytes" (4, 16, 512; 0 = one full chunk) -- tooling and tests. */
 int nvrx_crc_operator(uint32_t which, uint32_t* out_1024_words);
+
+/* ---- CRC-32 of extents at any offset and of any length, entirely on the device ----------------------------------------
+ * Verifies what a torch.distributed.checkpoint load put in HBM against the CRC-32 field of each storage record's ZIP
+ * directory entry (torch's writer fills it in; torch.load and FileSystemReader.read_data never check it).  The reference has
+ * no counterpart: its loads do not verify anything.  Unlike nvrx_crc_*, no host code reads payload bytes: the 16-byte
+ * aligned body of every extent goes through the same chunk kernel (whole 512-byte rows, 64 KiB chunks) and a second small
+ * kernel, one warp per extent, sums the head (< 16 bytes before the first 16-byte boundary) and the tail (< 512 bytes after
+ * the last whole row) and folds everything into the extent's crc32.  See csrc/crc_kernels.cuh.
+ *   offsets[i], nbytes[i]   extent i inside the buffer; any offset, any length (0 included); NVRX_E_INVALID on NULL arrays
+ *                           or offset + length overflow.  No CUDA call. */
+typedef struct nvrx_crcx nvrx_crcx;
+int nvrx_crcx_create(int64_t n, const uint64_t* offsets, const uint64_t* nbytes, int device, nvrx_crcx** out);
+int nvrx_crcx_destroy(nvrx_crcx* c);
+/* body chunks one run sums / kernel launches one run makes (1 with only sub-row extents, 2 otherwise, 0 when n == 0);
+ * either pointer may be NULL.  No CUDA call. */
+int nvrx_crcx_info(const nvrx_crcx* c, uint64_t* n_chunks, uint32_t* launches);
+/* Upload the descriptors on `stream` (otherwise done by the first run), e.g. to time the kernels alone. */
+int nvrx_crcx_commit(nvrx_crcx* c, void* stream);
+/* Enqueue on `stream`: when the stream reaches the end of this work, host_crcs[i] (pinned, n words; nothing past them is
+ * written) == zlib.crc32 of extent i of the buffer at dev_base (device memory, 16-byte aligned).  The buffer must stay
+ * unchanged until then.  The first run uploads the descriptors (stream-ordered). */
+int nvrx_crcx_run(nvrx_crcx* c, const void* dev_base, uint32_t* host_crcs, void* stream);
+/* zlib's crc32_combine: crc32(A | B) from crc32(A), crc32(B) and len(B) (any length below 2^64).  Returns the CRC, not a
+ * status; host only, no CUDA call.  Chains the parts of a record that was split over several staging batches. */
+uint32_t nvrx_crc32_combine(uint32_t crc_a, uint32_t crc_b, uint64_t len_b);
 
 #ifdef __cplusplus
 }

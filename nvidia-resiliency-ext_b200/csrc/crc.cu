@@ -248,6 +248,200 @@ int nvrx_crc_finish(int64_t n, const uint64_t* offsets, const uint64_t* nbytes, 
     return NVRX_OK;
 }
 
+// ---- extents at any offset and of any length, summed entirely on the device ------------------------------------------
+using nvrx::CrcxExtent;
+using nvrx::kCrcPow2Tables;
+
+namespace {
+
+// Z(2^k), k = 0..63, back to back: host copy (nvrx_crc32_combine) and one device copy per device (the fold kernel)
+const uint32_t* pow2_tables() {
+    static std::vector<uint32_t> t;
+    static std::once_flag once;
+    std::call_once(once, [] {
+        t.resize(static_cast<size_t>(kCrcPow2Tables) * kCrcOpWords);
+        memcpy(t.data(), ops().z1, sizeof(ops().z1));
+        for (uint32_t k = 1; k < kCrcPow2Tables; ++k) {
+            const uint32_t* prev = t.data() + (k - 1) * kCrcOpWords;
+            compose(prev, prev, t.data() + k * kCrcOpWords);
+        }
+    });
+    return t.data();
+}
+
+uint32_t* g_dev_pow2[64] = {nullptr};
+
+int device_pow2_tables(int device, uint32_t** out) {
+    if (device < 0 || device >= 64) return NVRX_E_INVALID;
+    std::lock_guard<std::mutex> lk(g_dev_lock);
+    if (!g_dev_pow2[device]) {
+        const size_t bytes = static_cast<size_t>(kCrcPow2Tables) * kCrcOpWords * sizeof(uint32_t);
+        uint32_t* d = nullptr;
+        NVRX_CUDA(cudaMalloc(&d, bytes));
+        const cudaError_t e = cudaMemcpy(d, pow2_tables(), bytes, cudaMemcpyHostToDevice);
+        if (e != cudaSuccess) {
+            cudaFree(d);
+            return static_cast<int>(e);
+        }
+        g_dev_pow2[device] = d;
+    }
+    *out = g_dev_pow2[device];
+    return NVRX_OK;
+}
+
+}  // namespace
+
+struct nvrx_crcx {
+    int device = 0;
+    int sm_count = 0;
+    std::vector<CrcxExtent> ext;
+    std::vector<CrcChunk> chunks;  // body chunks of all extents, extent by extent (ext[i].first indexes them)
+    uint8_t* d_mem = nullptr;      // [extents | chunks | chunk values | ready word | crcs], uploaded by the first run
+    size_t chunks_at = 0, vals_at = 0, ready_at = 0, out_at = 0;
+};
+
+int nvrx_crcx_create(int64_t n, const uint64_t* offsets, const uint64_t* nbytes, int device, nvrx_crcx** out) {
+    if (!out || n < 0 || n > 0xffffffffll || (n > 0 && (!offsets || !nbytes))) return NVRX_E_INVALID;
+    for (int64_t i = 0; i < n; ++i)
+        if (offsets[i] + nbytes[i] < offsets[i]) return NVRX_E_INVALID;
+    nvrx_crcx* c = new (std::nothrow) nvrx_crcx();
+    if (!c) return NVRX_E_NOMEM;
+    c->device = device;
+    try {
+        c->ext.resize(static_cast<size_t>(n));
+        for (int64_t i = 0; i < n; ++i) {
+            uint32_t head, tail;
+            uint64_t rows;
+            nvrx::crcx_split(offsets[i], nbytes[i], &head, &rows, &tail);
+            c->ext[i] = CrcxExtent{offsets[i], nbytes[i], c->chunks.size()};
+            uint64_t off = offsets[i] + head;
+            for (uint64_t k = 0, m = nvrx::crcx_chunks(rows); k < m; ++k) {
+                const uint32_t r = nvrx::crcx_chunk_rows(rows, k);
+                c->chunks.push_back(CrcChunk{off, r, static_cast<uint32_t>(i)});
+                off += static_cast<uint64_t>(r) * kCrcRowBytes;
+            }
+        }
+    } catch (const std::bad_alloc&) {
+        delete c;
+        return NVRX_E_NOMEM;
+    }
+    if (c->chunks.size() > 0xffffffffull) {
+        delete c;
+        return NVRX_E_INVALID;
+    }
+    *out = c;
+    return NVRX_OK;
+}
+
+int nvrx_crcx_destroy(nvrx_crcx* c) {
+    if (!c) return NVRX_OK;
+    if (c->d_mem) {
+        int prev = -1;
+        cudaGetDevice(&prev);
+        if (prev != c->device) cudaSetDevice(c->device);
+        cudaFree(c->d_mem);
+        if (prev >= 0 && prev != c->device) cudaSetDevice(prev);
+    }
+    delete c;
+    return NVRX_OK;
+}
+
+int nvrx_crcx_info(const nvrx_crcx* c, uint64_t* n_chunks, uint32_t* launches) {
+    if (!c) return NVRX_E_INVALID;
+    if (n_chunks) *n_chunks = c->chunks.size();
+    if (launches) *launches = (c->chunks.empty() ? 0u : 1u) + (c->ext.empty() ? 0u : 1u);
+    return NVRX_OK;
+}
+
+namespace {
+
+struct CrcxDevice {  // makes c->device current for the lifetime of the object
+    int prev = -1, dev = 0;
+    int enter(int d) {
+        dev = d;
+        NVRX_CUDA(cudaGetDevice(&prev));
+        if (prev != dev) NVRX_CUDA(cudaSetDevice(dev));
+        return NVRX_OK;
+    }
+    ~CrcxDevice() {
+        if (prev >= 0 && prev != dev) cudaSetDevice(prev);
+    }
+};
+
+int crcx_upload(nvrx_crcx* c, cudaStream_t st) {
+    const size_t n = c->ext.size(), nc = c->chunks.size();
+    if (!c->d_mem && n) {
+        NVRX_CUDA(cudaDeviceGetAttribute(&c->sm_count, cudaDevAttrMultiProcessorCount, c->device));
+        const auto up16 = [](size_t v) { return (v + 15) & ~static_cast<size_t>(15); };
+        c->chunks_at = up16(n * sizeof(CrcxExtent));
+        c->vals_at = up16(c->chunks_at + nc * sizeof(CrcChunk));
+        c->ready_at = up16(c->vals_at + nc * sizeof(uint32_t));
+        c->out_at = c->ready_at + 16;
+        NVRX_CUDA(cudaMalloc(&c->d_mem, c->out_at + n * sizeof(uint32_t)));
+        // stream-ordered from pageable memory: the runtime stages the descriptors before this call returns
+        NVRX_CUDA(cudaMemcpyAsync(c->d_mem, c->ext.data(), n * sizeof(CrcxExtent), cudaMemcpyHostToDevice, st));
+        if (nc)
+            NVRX_CUDA(cudaMemcpyAsync(c->d_mem + c->chunks_at, c->chunks.data(), nc * sizeof(CrcChunk), cudaMemcpyHostToDevice, st));
+    }
+    return NVRX_OK;
+}
+
+}  // namespace
+
+int nvrx_crcx_commit(nvrx_crcx* c, void* stream) {
+    if (!c) return NVRX_E_INVALID;
+    CrcxDevice guard;
+    int rc = guard.enter(c->device);
+    if (rc) return rc;
+    return crcx_upload(c, static_cast<cudaStream_t>(stream));
+}
+
+int nvrx_crcx_run(nvrx_crcx* c, const void* dev_base, uint32_t* host_crcs, void* stream) {
+    if (!c) return NVRX_E_INVALID;
+    const size_t n = c->ext.size(), nc = c->chunks.size();
+    if (!n) return NVRX_OK;
+    if (!host_crcs || !dev_base || (reinterpret_cast<uintptr_t>(dev_base) & 15u)) return NVRX_E_INVALID;
+    CrcxDevice guard;
+    int rc = guard.enter(c->device);
+    if (rc) return rc;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    rc = crcx_upload(c, st);
+    if (rc) return rc;
+    uint32_t *tables = nullptr, *pow2 = nullptr;
+    rc = device_tables(c->device, &tables);
+    if (!rc) rc = device_pow2_tables(c->device, &pow2);
+    if (rc) return rc;
+    const uint8_t* src = static_cast<const uint8_t*>(dev_base);
+    uint32_t* vals = reinterpret_cast<uint32_t*>(c->d_mem + c->vals_at);
+    uint32_t* crcs = reinterpret_cast<uint32_t*>(c->d_mem + c->out_at);
+    if (nc) {  // the bodies: the restore / snapshot checksum kernel, unchanged (its ready word goes to a scratch word)
+        constexpr int kWarps = 32;
+        NVRX_CUDA(cudaFuncSetAttribute(nvrx::crc_chunks_private<kWarps>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       static_cast<int>(nvrx::kCrcPrivateSmemBytes)));
+        const uint64_t want = (nc + kWarps - 1) / kWarps;
+        const uint32_t grid = static_cast<uint32_t>(want < static_cast<uint64_t>(c->sm_count) ? want : c->sm_count);
+        nvrx::crc_chunks_private<kWarps><<<grid, kWarps * 32, nvrx::kCrcPrivateSmemBytes, st>>>(
+            src, reinterpret_cast<const CrcChunk*>(c->d_mem + c->chunks_at), static_cast<uint32_t>(nc), tables, vals,
+            reinterpret_cast<unsigned long long*>(c->d_mem + c->ready_at), 0ull);
+        NVRX_CUDA(cudaGetLastError());
+    }
+    {
+        constexpr int kWarps = 8;
+        const uint64_t want = (n + kWarps - 1) / kWarps;
+        const uint64_t cap = static_cast<uint64_t>(c->sm_count) * 8;
+        const uint32_t grid = static_cast<uint32_t>(want < cap ? want : cap);
+        nvrx::crcx_fold<kWarps><<<grid, kWarps * 32, 0, st>>>(src, reinterpret_cast<const CrcxExtent*>(c->d_mem),
+                                                              static_cast<uint32_t>(n), vals, pow2, crcs);
+        NVRX_CUDA(cudaGetLastError());
+    }
+    NVRX_CUDA(cudaMemcpyAsync(host_crcs, crcs, n * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    return NVRX_OK;
+}
+
+uint32_t nvrx_crc32_combine(uint32_t crc_a, uint32_t crc_b, uint64_t len_b) {
+    return nvrx::crc_zeros(pow2_tables(), crc_a, len_b) ^ crc_b;
+}
+
 // Operator tables for tooling and tests: which = 4, 16, 512 -> Z(which); 0 -> Z(chunk bytes).  `out` holds 1024 words.
 int nvrx_crc_operator(uint32_t which, uint32_t* out) {
     if (!out) return NVRX_E_INVALID;

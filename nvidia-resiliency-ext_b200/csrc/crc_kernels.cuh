@@ -75,6 +75,83 @@ NVRX_HD uint32_t crc_fold_lane(const uint32_t* z4, const uint32_t t[4]) {
 // Chain step over lane values that sit 16 bytes apart: s <- Z(16)(s) ^ u.
 NVRX_HD uint32_t crc_chain_lane(const uint32_t* z16, uint32_t s, uint32_t u) { return crc_apply(z16, s) ^ u; }
 
+// ---- extents at any offset and of any length (nvrx_crcx_*) ----------------------------------------------------------
+// An extent [off, off + len) of a 16-byte aligned buffer splits into
+//     head  [off, a)                  a = min(round_up(off, 16), off + len): fewer than 16 bytes, summed byte by byte
+//     body  [a, a + 512 * rows)       whole rows, in chunks of kCrcChunkRows rows: the values crc_chunks_private<> makes
+//     tail  [a + 512 * rows, end)     fewer than 512 bytes, starting 16-byte aligned: 16 bytes per lane, like a short row
+// and its crc32 is ~(Z(tail)(Z(body)(head state) ^ body value) ^ tail value), the head state fed from 0xFFFFFFFF.
+// Z(n) for any n is applied through the tables Z(2^k), k = 0..63 (pow2 + k * kCrcOpWords): one lookup round per set bit.
+constexpr uint32_t kCrcPow2Tables = 64;
+
+struct CrcxExtent {
+    uint64_t off;    // byte offset inside the buffer (any alignment)
+    uint64_t len;    // bytes (0 allowed)
+    uint64_t first;  // index of the extent's first body chunk value
+};
+
+NVRX_HD void crcx_split(uint64_t off, uint64_t len, uint32_t* head, uint64_t* rows, uint32_t* tail) {
+    const uint64_t h = (16u - (off & 15u)) & 15u;
+    *head = static_cast<uint32_t>(h < len ? h : len);
+    const uint64_t rest = len - *head;
+    *rows = rest / kCrcRowBytes;
+    *tail = static_cast<uint32_t>(rest % kCrcRowBytes);
+}
+
+// body chunks of an extent with `rows` whole rows, and the rows of its last chunk
+NVRX_HD uint64_t crcx_chunks(uint64_t rows) { return (rows + kCrcChunkRows - 1) / kCrcChunkRows; }
+NVRX_HD uint32_t crcx_chunk_rows(uint64_t rows, uint64_t c) {
+    const uint64_t left = rows - c * kCrcChunkRows;
+    return static_cast<uint32_t>(left < kCrcChunkRows ? left : kCrcChunkRows);
+}
+
+// Z(n)(s) for any n (zlib's crc32_combine: crc(A | B) = Z(len B)(crc A) ^ crc B).
+NVRX_HD uint32_t crc_zeros(const uint32_t* pow2, uint32_t s, uint64_t n) {
+    for (uint32_t k = 0; n; ++k, n >>= 1)
+        if (n & 1u) s = crc_apply(pow2 + k * kCrcOpWords, s);
+    return s;
+}
+
+// Feed n bytes into state s one at a time (z1 = Z(1): its first 256 words are the classic byte table).
+NVRX_HD uint32_t crc_feed_bytes(const uint32_t* z1, uint32_t s, const uint8_t* p, uint32_t n) {
+    for (uint32_t k = 0; k < n; ++k) s = z1[(s ^ p[k]) & 0xffu] ^ (s >> 8);
+    return s;
+}
+
+// Lane `lane` of 32 folds the contiguous block of chunk values [begin, end) it owns: value and byte count of the block.
+NVRX_HD void crcx_lane_block(uint64_t n_chunks, uint32_t lane, uint64_t* begin, uint64_t* end) {
+    const uint64_t q = (n_chunks + 31u) / 32u;
+    const uint64_t b = lane * q;
+    *begin = b < n_chunks ? b : n_chunks;
+    *end = b + q < n_chunks ? b + q : n_chunks;
+}
+NVRX_HD uint32_t crcx_fold_block(const uint32_t* pow2, const uint32_t* vals, uint64_t rows, uint64_t begin, uint64_t end,
+                                 uint64_t* bytes) {
+    uint32_t u = 0;
+    uint64_t nb = 0;
+    for (uint64_t c = begin; c < end; ++c) {
+        const uint64_t cb = static_cast<uint64_t>(crcx_chunk_rows(rows, c)) * kCrcRowBytes;
+        u = crc_zeros(pow2, u, cb) ^ vals[c];
+        nb += cb;
+    }
+    *bytes = nb;
+    return u;
+}
+
+// Lane `lane`'s share of a tail of `tail` bytes at p: bytes [16 lane, 16 lane + 16) of it, value from state 0.
+NVRX_HD uint32_t crcx_tail_lane(const uint32_t* z1, const uint8_t* p, uint32_t tail, uint32_t lane, uint32_t* n) {
+    const uint32_t b = 16u * lane;
+    *n = b < tail ? (tail - b < 16u ? tail - b : 16u) : 0u;
+    return crc_feed_bytes(z1, 0u, p + b, *n);
+}
+
+// The extent's crc32 from its head state and the body and tail values.
+NVRX_HD uint32_t crcx_finish(const uint32_t* pow2, uint32_t head_state, uint64_t rows, uint32_t body, uint32_t tail_bytes,
+                             uint32_t tail) {
+    const uint32_t s = crc_zeros(pow2, head_state, rows * kCrcRowBytes) ^ body;
+    return ~(crc_zeros(pow2, s, tail_bytes) ^ tail);
+}
+
 #if defined(__CUDACC__)
 
 // tables: [Z512 | Z4 | Z16], kCrcOpWords each, in global memory; copied to shared memory once per CTA.
@@ -161,6 +238,38 @@ crc_chunks_private(const uint8_t* __restrict__ base, const CrcChunk* __restrict_
 #pragma unroll
         for (int l = 0; l < 32; ++l) s = crc_chain_lane(z16, s, __shfl_sync(0xffffffffu, u, l));
         if (lane == 0) out[c] = s;
+    }
+}
+
+// Second pass of nvrx_crcx_run: one warp per extent folds the body chunk values crc_chunks_private<> left in `vals` (a
+// contiguous block per lane, then the 32 block values chained), sums the head and the tail from `base` and writes the
+// extent's crc32 to out[i].  pow2: the tables Z(2^k), read through L1 (a few hundred lookups per extent).
+template <int WARPS>
+__global__ void __launch_bounds__(WARPS * 32)
+crcx_fold(const uint8_t* __restrict__ base, const CrcxExtent* __restrict__ ext, uint32_t n,
+          const uint32_t* __restrict__ vals, const uint32_t* __restrict__ pow2, uint32_t* __restrict__ out) {
+    const uint32_t lane = threadIdx.x & 31u;
+    const uint32_t warp = blockIdx.x * WARPS + (threadIdx.x >> 5);
+    const uint32_t n_warps = gridDim.x * WARPS;
+    for (uint32_t i = warp; i < n; i += n_warps) {
+        const CrcxExtent e = ext[i];
+        uint32_t head, tail;
+        uint64_t rows;
+        crcx_split(e.off, e.len, &head, &rows, &tail);
+        uint64_t b, en, nb;
+        crcx_lane_block(crcx_chunks(rows), lane, &b, &en);
+        const uint32_t u = crcx_fold_block(pow2, vals + e.first, rows, b, en, &nb);
+        uint32_t tn;
+        const uint32_t w = crcx_tail_lane(pow2, base + e.off + head + rows * kCrcRowBytes, tail, lane, &tn);
+        uint32_t body = 0, tv = 0;
+        for (int l = 0; l < 32; ++l) {  // every lane chains all 32 (uniform control flow); lane 0 stores
+            body = crc_zeros(pow2, body, __shfl_sync(0xffffffffu, nb, l)) ^ __shfl_sync(0xffffffffu, u, l);
+            tv = crc_zeros(pow2, tv, __shfl_sync(0xffffffffu, tn, l)) ^ __shfl_sync(0xffffffffu, w, l);
+        }
+        if (lane == 0) {
+            const uint32_t hs = crc_feed_bytes(pow2, 0xffffffffu, base + e.off, head);
+            out[i] = crcx_finish(pow2, hs, rows, body, tail, tv);
+        }
     }
 }
 

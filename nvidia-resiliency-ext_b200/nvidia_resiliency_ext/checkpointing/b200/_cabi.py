@@ -12,7 +12,7 @@ import os
 from pathlib import Path
 from typing import Optional
 
-ABI_VERSION = 4
+ABI_VERSION = 5
 
 OK = 0
 E_INVALID = 1000
@@ -105,6 +105,12 @@ EXPORTED_SYMBOLS = (
     "nvrx_crc_run",
     "nvrx_crc_finish",
     "nvrx_crc_operator",
+    "nvrx_crcx_create",
+    "nvrx_crcx_destroy",
+    "nvrx_crcx_info",
+    "nvrx_crcx_commit",
+    "nvrx_crcx_run",
+    "nvrx_crc32_combine",
 )
 
 
@@ -113,10 +119,14 @@ class SnapError(RuntimeError):
 
     def __init__(self, status: int, what: str, detail: str = ""):
         self.status = status
+        self._args = (status, what, detail)
         msg = f"{what} failed with status {status}"
         if detail:
             msg += f" ({detail})"
         super().__init__(msg)
+
+    def __reduce__(self):  # picklable: torch.distributed.checkpoint gathers a rank's exception across ranks
+        return type(self), self._args
 
 
 def library_path() -> Path:
@@ -210,6 +220,12 @@ def _declare(lib: C.CDLL) -> None:
         "nvrx_crc_run": (_int, [_vp, _vp, _vp, _vp, _u64, _vp]),
         "nvrx_crc_finish": (_int, [_i64, P(_u64), P(_u64), _vp, _u64, _vp, P(_u32)]),
         "nvrx_crc_operator": (_int, [_u32, P(_u32)]),
+        "nvrx_crcx_create": (_int, [_i64, P(_u64), P(_u64), _int, P(_vp)]),
+        "nvrx_crcx_destroy": (_int, [_vp]),
+        "nvrx_crcx_info": (_int, [_vp, P(_u64), P(_u32)]),
+        "nvrx_crcx_commit": (_int, [_vp, _vp]),
+        "nvrx_crcx_run": (_int, [_vp, _vp, _vp, _vp]),
+        "nvrx_crc32_combine": (_u32, [_u32, _u32, _u64]),
     }
     assert set(sigs) == set(EXPORTED_SYMBOLS)
     for name, (res, args) in sigs.items():

@@ -278,6 +278,69 @@ class CrcPlan:
             pass
 
 
+class CrcxPlan:
+    """Extents at any offset and of any length of a device buffer whose zlib CRC-32s the GPU computes entirely
+    (``nvrx_crcx_*``): ``run`` enqueues the kernels and the copy of one crc32 per extent into pinned host memory.  Creating
+    it is CUDA-free."""
+
+    def __init__(self, offsets: Sequence[int], nbytes: Sequence[int], device: int):
+        self._lib = _cabi.lib()
+        self._h = C.c_void_p()
+        self.n = len(offsets)
+        check(self._lib.nvrx_crcx_create(self.n, _u64_array(offsets), _u64_array(nbytes), device, C.byref(self._h)), "nvrx_crcx_create")
+        chunks, launches = C.c_uint64(), C.c_uint32()
+        check(self._lib.nvrx_crcx_info(self._h, C.byref(chunks), C.byref(launches)), "nvrx_crcx_info")
+        self.n_chunks, self.launches = chunks.value, launches.value
+
+    def commit(self, stream: int) -> None:
+        check(self._lib.nvrx_crcx_commit(self._h, stream), "nvrx_crcx_commit")
+
+    def run(self, dev_base: int, host_crcs: int, stream: int) -> None:
+        check(self._lib.nvrx_crcx_run(self._h, dev_base, host_crcs, stream), "nvrx_crcx_run")
+
+    def close(self) -> None:
+        if self._h:
+            self._lib.nvrx_crcx_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def crc32_combine(crc_a: int, crc_b: int, len_b: int) -> int:
+    """zlib's ``crc32_combine``: crc32(A + B) from crc32(A), crc32(B) and len(B) (``nvrx_crc32_combine``, host only)."""
+    return int(_cabi.lib().nvrx_crc32_combine(crc_a, crc_b, len_b))
+
+
+def record_verify_ranges(spans: Sequence[Tuple[int, int]], length: int, limit: int):
+    """Read ranges that check a record of ``length`` bytes in full while reading the byte spans ``[a, b)`` its load pieces
+    need.  Returns ``(ranges, whole)``: ``ranges[k] = (r, e)`` is piece k's read range, ``r <= a_k`` and ``e >= b_k``; with
+    the pieces sorted by span, piece k reads from the end of piece k-1's range (0 for the first) to the start of piece
+    k+1's span (``length`` for the last), so the ranges tile ``[0, length)`` and nothing is read twice -- spans that already
+    tile the record add no byte.  ``whole``: extra ranges read for the checksum alone, each at most ``limit`` bytes: the
+    parts of a gap that would make a piece's range longer than ``limit``.  When two spans overlap the rule cannot tile
+    them: ``ranges`` is None (the pieces read their spans only) and ``whole`` covers the record once more."""
+    order = sorted(range(len(spans)), key=lambda k: spans[k])
+    parts = lambda lo, hi: [(p, min(p + limit, hi)) for p in range(lo, hi, limit)]  # noqa: E731
+    if any(spans[order[j + 1]][0] < spans[order[j]][1] for j in range(len(order) - 1)):
+        return None, parts(0, length)
+    ranges: List[Optional[Tuple[int, int]]] = [None] * len(spans)
+    whole, start = [], 0
+    for j, k in enumerate(order):
+        a, b = spans[k]
+        end = spans[order[j + 1]][0] if j + 1 < len(order) else length
+        if end - start <= limit:
+            ranges[k] = (start, end)
+        else:  # the gaps travel on their own, in parts that fit a batch
+            ranges[k] = (a, b)
+            whole += parts(start, a) + parts(b, end)
+        start = end
+    return ranges, whole
+
+
 # (saved dtype, target dtype) -> nvrx_boxplan_create_cast code: the conversions the box scatter makes on the way
 BOX_CASTS = {
     (torch.float32, torch.bfloat16): _cabi.CAST_F32_BF16,
@@ -360,7 +423,11 @@ class BoxLoad(NamedTuple):
     ``file_off`` / ``file_len``: where the chunk's storage bytes sit in ``path``; ``src_offset`` / ``src_strides``: element
     offset of the sub-box's first element in that storage and the chunk's strides (elements).  The box's sizes are
     ``target.shape``.  ``src_dtype``: the chunk's dtype when it differs from the target's (fp32 / bf16 / fp16 into another
-    of the three, converted on the device); None means the target's dtype."""
+    of the three, converted on the device); None means the target's dtype.
+
+    For ``load_boxes(verify=True)``: ``record_crc`` is the CRC-32 of the storage record that starts at ``file_off`` (its ZIP
+    directory field; 0 = written without checksums, None = nothing to check), ``record_len`` its byte length (default
+    ``file_len``) and ``name`` what an error message calls the item (its fqn)."""
 
     path: str
     file_off: int
@@ -369,6 +436,9 @@ class BoxLoad(NamedTuple):
     src_strides: Tuple[int, ...]
     target: torch.Tensor
     src_dtype: Optional[torch.dtype] = None
+    record_crc: Optional[int] = None
+    record_len: Optional[int] = None
+    name: str = ""
 
 
 def box_span(sizes: Sequence[int], strides: Sequence[int], elem: int) -> int:
@@ -1248,7 +1318,7 @@ class SnapshotEngine:
     # staging bytes one batch of load_boxes() may use (the buffer is reused by every batch)
     DCP_LOAD_STAGING = int(os.environ.get("NVRX_B200_DCP_LOAD_STAGING_MB", "2048")) << 20
 
-    def load_boxes(self, entries: Sequence[BoxLoad]) -> None:
+    def load_boxes(self, entries: Sequence[BoxLoad], *, verify: bool = False) -> None:
         """Resharded load: write the sub-box of a saved chunk described by every entry into its target view (a CUDA tensor of
         this device, any strides, the chunk's dtype or -- fp32 / bf16 / fp16 into another of the three, ``src_dtype`` --
         converted on the way).  Blocking, like ``restore``.
@@ -1257,12 +1327,21 @@ class SnapshotEngine:
         file per batch) to a staging position that lines up with the target's first byte (``box_stage_pos``), so that
         same-layout loads are aligned vector copies or conversions; one ``nvrx_box_scatter`` per batch writes the views.  Batches hold at most
         ``DCP_LOAD_STAGING`` bytes and reuse one buffer: batch k+1's copies are enqueued on the stream after batch k's
-        scatter.  An entry larger than a batch is cut along its outermost dim (down to element ranges of a single run)."""
+        scatter.  An entry larger than a batch is cut along its outermost dim (down to element ranges of a single run).
+
+        ``verify=True``: every storage record an entry reads bytes from and whose ``record_crc`` is set is checked in full,
+        once, against that CRC-32 -- over the bytes as stored (before any conversion), as they arrived in staging.  The read
+        ranges of a record grow to tile it (``record_verify_ranges``; nothing extra when the pieces' spans already tile it),
+        ``nvrx_crcx_run`` sums each batch's ranges on the stream after that batch's fills, and the host chains a record's
+        parts in file order (``crc32_combine``).  A mismatch raises ``SnapError`` ("crc32 mismatch ...") after the load;
+        the targets may then hold the unverified bytes.  A non-empty record whose CRC field is 0 (written without checksums)
+        is counted in ``last_box_load["unverified_records"]`` and not checked."""
         import time as _time
 
         budget = max(int(self.DCP_LOAD_STAGING), 4096)
         # pieces: (path, file offset of the span, span bytes, box tuple without staging offset + cast code + (es, ed, V))
         pieces = []
+        records: Dict[Tuple[str, int], list] = {}  # verify: (path, record offset) -> [crc, length, names, piece indices]
         for e in entries:
             t = e.target
             if not (t.is_cuda and t.get_device() == self.device):
@@ -1288,22 +1367,52 @@ class SnapshotEngine:
             for sz, so, do in split_box(sizes, e.src_offset, sstr, 0, dstr, es, budget - 16):
                 dst = t.data_ptr() + do * ed
                 pieces.append((e.path, e.file_off + so * es, box_span(sz, sstr, es), (es, sz, sstr, dst, dstr, cast, conv)))
+                if verify and e.record_crc is not None:
+                    rec = records.setdefault(
+                        (e.path, e.file_off), [int(e.record_crc), e.file_len if e.record_len is None else int(e.record_len), [], []]
+                    )
+                    if e.name not in rec[2]:
+                        rec[2].append(e.name)
+                    rec[3].append(len(pieces) - 1)
+        # units: (path, file offset, bytes, head, box or None, checksum tag).  A unit reads [file offset, + bytes); its box's
+        # span starts `head` bytes in.  Tagged units (record key, offset in the record) are summed for their record.
+        units = [(path, off, nb, 0, box, None) for path, off, nb, box in pieces]
+        verified, unverified, extra = [], 0, 0
+        t_verify = _time.perf_counter()
+        for key, (crc, length, _, idx) in records.items():
+            if crc == 0:
+                unverified += 1  # written without checksums
+                continue
+            verified.append(key)
+            spans = [(pieces[k][1] - key[1], pieces[k][1] - key[1] + pieces[k][2]) for k in idx]
+            ranges, whole = record_verify_ranges(spans, length, budget - 16)
+            if ranges is not None:
+                for (a, _), k, (r, e_) in zip(spans, idx, ranges):
+                    units[k] = (key[0], key[1] + r, e_ - r, a - r, pieces[k][3], (key, r))
+            units += [(key[0], key[1] + r, e_ - r, 0, None, (key, r)) for r, e_ in whole]
+            extra += sum(e_ - r for r, e_ in whole) + (0 if ranges is None else sum(e_ - r for r, e_ in ranges) - sum(b - a for a, b in spans))
+        verify_s = _time.perf_counter() - t_verify  # host time of the verify path: range planning, CRC plans, chaining
         # one nvrx_fill_from_fd per file per batch copies each ring chunk from its file's first to its last byte in it, gaps
         # included: the pieces of a file must occupy one staging range of their own, so they are placed file by file (and in
         # file order, which also keeps the reads sequential)
-        pieces.sort(key=lambda pc: (pc[0], pc[1]))
-        # batches: a piece starts at the first position >= the cursor that box_stage_pos allows (at most 15 bytes later)
+        units.sort(key=lambda u: (u[0], u[1]))
+        # batches: a box's span starts at the first position >= the cursor (+ its unit's head) that box_stage_pos allows (at
+        # most 15 bytes later); a unit read for its checksum alone goes at the cursor
+        place = lambda c, u: box_stage_pos(c + u[3], u[4][3], u[4][6]) - u[3] if u[4] is not None else c  # noqa: E731
         batches, cur = [[]], 0
-        for piece in pieces:
-            pos = box_stage_pos(cur, piece[3][3], piece[3][6])
-            if batches[-1] and pos + piece[2] > budget:
+        for u in units:
+            pos = place(cur, u)
+            if batches[-1] and pos + u[2] > budget:
                 batches.append([])
-                pos = box_stage_pos(0, piece[3][3], piece[3][6])
-            batches[-1].append((pos,) + piece)
-            cur = pos + piece[2]
+                pos = place(0, u)
+            batches[-1].append((pos,) + u)
+            cur = pos + u[2]
         batches = [b for b in batches if b]
         peak = max((b[-1][0] + b[-1][3] for b in batches), default=0)
         stats = {"batches": len(batches), "peak_staging_bytes": peak, "algorithmic_bytes": 0, "box_ms": 0.0 if self.timing else None}
+        if verify:
+            stats.update(verified_records=len(verified), unverified_records=unverified, verify_extra_bytes=extra,
+                         crc_bytes=0, crc_ms=0.0 if self.timing else None, verify_host_ms=0.0)
         self.box_loads += 1
         self.last_box_load = stats
         if not batches:
@@ -1314,12 +1423,12 @@ class SnapshotEngine:
             stream_wait_event(stream, self._staging_free)
         threads = self.RESTORE_THREADS or max(self.prefault_threads, min(32, os.cpu_count() or 1))
         fds: Dict[str, int] = {}
-        plans, timers = [], []
+        plans, timers, crc_runs, crc_timers = [], [], [], []
         t0 = _time.perf_counter()
         try:
             for batch in batches:
                 by_file: Dict[str, list] = {}
-                for pos, path, file_off, nbytes, _ in batch:
+                for pos, path, file_off, nbytes, _, _, _ in batch:
                     by_file.setdefault(path, []).append((pos, nbytes, file_off))
                 end = batch[-1][0] + batch[-1][3]
                 for path, ext in by_file.items():
@@ -1333,22 +1442,42 @@ class SnapshotEngine:
                         ),
                         "nvrx_fill_from_fd",
                     )
-                plan = BoxPlan(
-                    [(b[0], b[1], pos, b[2], b[3], b[4]) for pos, _, _, _, b in batch], end, device=self.device,
-                    casts=[b[5] for _, _, _, _, b in batch],
-                )
-                plans.append(plan)
-                stats["algorithmic_bytes"] += plan.algorithmic_bytes
-                if self.timing:
-                    plan.commit(stream)  # descriptor upload outside the timed window: the events bracket the kernel
-                    ev = (Event(self.device, timing=True), Event(self.device, timing=True))
-                    ev[0].record(stream)
-                plan.scatter(staging.ptr, stream)
-                if self.timing:
-                    ev[1].record(stream)
-                    timers.append(ev)
-                self.launches += plan.launches
+                boxed = [(pos + head, b) for pos, _, _, _, head, b, _ in batch if b is not None]
+                if boxed:  # (only a batch of checksum-only reads has no box)
+                    plan = BoxPlan(
+                        [(b[0], b[1], pos, b[2], b[3], b[4]) for pos, b in boxed], end, device=self.device,
+                        casts=[b[5] for _, b in boxed],
+                    )
+                    plans.append(plan)
+                    stats["algorithmic_bytes"] += plan.algorithmic_bytes
+                    if self.timing:
+                        plan.commit(stream)  # descriptor upload outside the timed window: the events bracket the kernel
+                        ev = (Event(self.device, timing=True), Event(self.device, timing=True))
+                        ev[0].record(stream)
+                    plan.scatter(staging.ptr, stream)
+                    if self.timing:
+                        ev[1].record(stream)
+                        timers.append(ev)
+                    self.launches += plan.launches
                 self.box_batches += 1
+                tagged = [(pos, nbytes, tag) for pos, _, _, nbytes, _, _, tag in batch if tag is not None]
+                if tagged:
+                    # same stream: after this batch's fills, before the next batch's fills overwrite staging
+                    t_verify = _time.perf_counter()
+                    crc = CrcxPlan([x[0] for x in tagged], [x[1] for x in tagged], self.device)
+                    host = torch.zeros(len(tagged), dtype=torch.int32).pin_memory()
+                    crc_runs.append((crc, host, tagged))
+                    stats["crc_bytes"] += sum(x[1] for x in tagged)
+                    if self.timing:
+                        crc.commit(stream)
+                        ev = (Event(self.device, timing=True), Event(self.device, timing=True))
+                        ev[0].record(stream)
+                    crc.run(staging.ptr, host.data_ptr(), stream)
+                    if self.timing:
+                        ev[1].record(stream)
+                        crc_timers.append(ev)
+                    self.launches += crc.launches
+                    verify_s += _time.perf_counter() - t_verify
             done = Event(self.device)
             done.record(stream)
             self._staging_free = done
@@ -1360,8 +1489,46 @@ class SnapshotEngine:
             plan.close()
         if timers:
             stats["box_ms"] = sum(a.elapsed_ms(b) for a, b in timers)
+        if crc_timers:
+            stats["crc_ms"] = sum(a.elapsed_ms(b) for a, b in crc_timers)
         if self.trace is not None:
             self.trace["load_boxes"] = {"wall_s": _time.perf_counter() - t0}
+        if crc_runs:
+            t_verify = _time.perf_counter()
+            try:
+                self._check_record_crcs(records, crc_runs)
+            finally:
+                stats["verify_host_ms"] = (verify_s + _time.perf_counter() - t_verify) * 1e3
+        elif verify:
+            stats["verify_host_ms"] = verify_s * 1e3
+
+    def _check_record_crcs(self, records: Dict[Tuple[str, int], list], crc_runs: list) -> None:
+        """Chain the parts of every verified record in file order and raise on the first records that do not match."""
+        parts: Dict[Tuple[str, int], list] = {}
+        for crc, host, tagged in crc_runs:
+            vals = [v & 0xFFFFFFFF for v in host.tolist()]  # int32 bits -> uint32
+            for (_, nbytes, (key, r)), v in zip(tagged, vals):
+                parts.setdefault(key, []).append((r, nbytes, v))
+            crc.close()
+        bad = []
+        for key, ps in parts.items():
+            ps.sort()
+            got = ps[0][2]  # a record read in one part (the common case) needs no combine
+            for _, nbytes, v in ps[1:]:
+                got = crc32_combine(got, v, nbytes)
+            if got != records[key][0]:
+                bad.append((key, got))
+        if bad:
+            detail = "; ".join(
+                f"{', '.join(records[key][2]) or '?'} in {key[0]} at record offset {key[1]}: got {got:#010x}, "
+                f"file says {records[key][0]:#010x}"
+                for key, got in bad[:4]
+            )
+            raise SnapError(
+                _cabi.E_STATE, "verifying loaded items",
+                f"crc32 mismatch on {len(bad)} of {len(parts)} records ({detail}) -- the checkpoint or the path it came "
+                "through is corrupt; the targets hold the unverified bytes",
+            )
 
     def resident_source(self, path, host_tensors: Sequence[torch.Tensor]) -> Optional[Tuple[_Slot, List[int]]]:
         """``(slot, payload offsets)`` when the checkpoint file ``path`` is a hard link to one of this engine's live,

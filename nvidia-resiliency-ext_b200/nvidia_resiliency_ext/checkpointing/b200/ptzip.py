@@ -566,6 +566,8 @@ class SavedChunk:
     storage_offset: int
     size: Tuple[int, ...]
     stride: Tuple[int, ...]
+    crc32: int = 0  # the record's CRC-32 field in the central directory (0 on a non-empty record: written without one)
+    record_len: int = 0  # byte length of the record (>= the storage's bytes)
 
 
 class _TensorRecordUnpickler(pickle.Unpickler):
@@ -594,12 +596,36 @@ class _TensorRecordUnpickler(pickle.Unpickler):
         return ("storage", pid[1][1], str(pid[2]), int(pid[4]))
 
 
+class RecordChecksumError(ValueError):
+    """A member of a tensor archive whose bytes do not match its CRC-32 field (the same message zipfile gives)."""
+
+    def __init__(self, member: str, header_off: int, got: int, expected: int):
+        self.member, self.header_off, self.got, self.expected = member, header_off, got, expected
+        super().__init__(f"not a single-tensor torch.save archive: Bad CRC-32 for file {member!r}")
+
+    def __reduce__(self):  # picklable: torch.distributed.checkpoint gathers a rank's exception across ranks
+        return type(self), (self.member, self.header_off, self.got, self.expected)
+
+
+def _stored_payload(fd: int, offset: int, info) -> bytes:
+    """The bytes of an uncompressed member ``info`` of the archive embedded at ``offset`` of ``fd``."""
+    hdr = os.pread(fd, 30, offset + info.header_offset)
+    if len(hdr) != 30 or hdr[:4] != b"PK\x03\x04":
+        raise ValueError(f"bad local header of {info.filename}")
+    name_len, extra_len = struct.unpack_from("<HH", hdr, 26)
+    data = os.pread(fd, info.file_size, offset + info.header_offset + 30 + name_len + extra_len)
+    if len(data) != info.file_size:
+        raise ValueError(f"{info.filename} is truncated")
+    return data
+
+
 def read_tensor_record(fd: int, offset: int, length: int) -> SavedChunk:
     """Describe the ``torch.save`` archive of ONE tensor embedded at ``[offset, offset + length)`` of ``fd`` (how
     ``torch.distributed.checkpoint`` stores every tensor item of a ``.distcp`` file): where its payload starts, its dtype,
-    element count, storage offset, size and stride (any strides: a chunk that was not cloned keeps them).  Reads the
-    directory and ``data.pkl`` only -- not the payload -- and never runs code from the pickle; ``ValueError`` when the
-    window is not such an archive."""
+    element count, storage offset, size and stride (any strides: a chunk that was not cloned keeps them), and the storage
+    record's CRC-32 field and byte length.  Reads the directory and ``data.pkl`` only -- not the payload -- and never runs
+    code from the pickle; ``ValueError`` when the window is not such an archive, ``RecordChecksumError`` (a ValueError)
+    when ``data.pkl`` does not match its non-zero CRC-32 field."""
     import zipfile
 
     try:
@@ -608,7 +634,12 @@ def read_tensor_record(fd: int, offset: int, length: int) -> SavedChunk:
             pkl = [i for i in zf.infolist() if i.filename.endswith("/data.pkl") and i.filename.count("/") == 1]
             if len(pkl) != 1:
                 raise ValueError("no data.pkl record")
-            rec = _TensorRecordUnpickler(io.BytesIO(zf.read(pkl[0]))).load()
+            # read the stored pickle directly and check it against its CRC-32 field like zipfile does, except when the field
+            # is 0: an archive written with torch.serialization.set_crc32_options(False) (torch.load accepts those)
+            pkl_bytes = _stored_payload(fd, offset, pkl[0]) if pkl[0].compress_type == zipfile.ZIP_STORED else zf.read(pkl[0])
+            if pkl[0].CRC and zlib.crc32(pkl_bytes) != pkl[0].CRC:
+                raise RecordChecksumError(pkl[0].filename, offset + pkl[0].header_offset, zlib.crc32(pkl_bytes), pkl[0].CRC)
+            rec = _TensorRecordUnpickler(io.BytesIO(pkl_bytes)).load()
             if not (isinstance(rec, tuple) and rec[0] == "tensor" and rec[2][0] == "storage"):
                 raise ValueError("data.pkl does not describe a single tensor")
             _, fn, (_, st_dtype, key, st_numel), st_off, size, stride, rest = rec
@@ -634,4 +665,5 @@ def read_tensor_record(fd: int, offset: int, length: int) -> SavedChunk:
             data_off = offset + info.header_offset + 30 + name_len + extra_len
     except (zipfile.BadZipFile, pickle.UnpicklingError, EOFError, TypeError, IndexError) as e:
         raise ValueError(f"not a single-tensor torch.save archive: {e}") from e
-    return SavedChunk(data_off=data_off, dtype=dtype, numel=int(st_numel), storage_offset=int(st_off), size=size, stride=stride)
+    return SavedChunk(data_off=data_off, dtype=dtype, numel=int(st_numel), storage_offset=int(st_off), size=size, stride=stride,
+                      crc32=int(info.CRC), record_len=int(info.file_size))
