@@ -681,6 +681,15 @@ class _Slot:
     busy: bool = False
     drained_total: int = 0  # cumulative bytes the progress word has been advanced by
     done_event: Optional[Event] = None
+    crc_done: Optional[Event] = None  # the last GPU-checksum run's values and ready word have landed in the buffer
+
+    def wait_device_writes(self) -> None:
+        """Block until every device copy into the buffer has landed: the last drain and, with GPU checksums, the last
+        checksum values and ready word.  A released slot may still have them queued (an aborted or failed save), so a host
+        writer or closing the buffer must come after this."""
+        for ev in (self.done_event, self.crc_done):
+            if ev is not None:
+                ev.synchronize()
 
     def published(self) -> bool:
         """A checkpoint file is a hard link to this slot (zero-copy persistence): its pages must not be overwritten."""
@@ -898,13 +907,17 @@ class SnapshotEngine:
             self._staging = DeviceBuffer(max(nbytes, 512), self.device)
         return self._staging
 
-    def _acquire_slot(self, nbytes: int, slot: Optional[_Slot] = None) -> _Slot:
+    def _acquire_slot(self, nbytes: int, slot: Optional[_Slot] = None, *, host_write: bool = False) -> _Slot:
+        """A slot of at least ``nbytes`` for the caller.  ``host_write``: the caller fills it on the host, so the device
+        copies a released save may still have queued into it are waited for first.  A snapshot needs no wait: its drain
+        runs on the side stream after the earlier ones."""
         if slot is None:
             slot, retire = choose_slot(self._slots, nbytes, self.max_host_slots)
             if retire:
                 # the pool is full of checkpoints somebody keeps: give this one up (the file keeps the pages, this process
                 # drops its mapping and pinning) and start a fresh buffer in its place
                 slot.__dict__.pop("_exchange_views", None)
+                slot.wait_device_writes()
                 slot.buf.close()
                 slot.buf = None
         if slot is None and len(self._slots) < self.max_host_slots:
@@ -922,6 +935,7 @@ class SnapshotEngine:
         if slot.buf is None or slot.buf.capacity < nbytes:
             slot.__dict__.pop("_exchange_views", None)  # cached host views of the old buffer (b200/exchange.py)
             if slot.buf is not None:
+                slot.wait_device_writes()  # unregistering and unmapping under a queued copy would be a use-after-free
                 slot.buf.close()
             self._slot_gen += 1
             name = f"{self.shm_prefix}_s{slot.index}_g{self._slot_gen}"
@@ -929,6 +943,8 @@ class SnapshotEngine:
                 nbytes, name=name, pin=True, device=self.device, prefault_threads=self.prefault_threads
             )
             slot.drained_total = 0
+        elif host_write:
+            slot.wait_device_writes()
         if slot.done_event is None:
             slot.done_event = Event(self.device)
         slot.busy = True
@@ -1103,6 +1119,7 @@ class SnapshotEngine:
             self.launches += 1
             crc_done = Event(self.device)
             crc_done.record(self._aux.handle)
+            slot.crc_done = crc_done  # the values and the ready word are device copies into the slot, too
             # staging is free for the next pack only when the drain AND the checksum kernel are through with it
             self._side.wait_event(crc_done)
             free_ev = Event(self.device)
@@ -1189,7 +1206,7 @@ class SnapshotEngine:
             self.resident_restores += 1
         else:
             plan = self._plan_for(out, mask)
-            slot = self._acquire_slot(plan.staging_bytes)
+            slot = self._acquire_slot(plan.staging_bytes, host_write=True)  # gathered or read into below
         staging = self._ensure_staging(plan.staging_bytes)
         try:
             if resident is None and file_source is not None:
@@ -1566,8 +1583,7 @@ class SnapshotEngine:
             self._staging = None
         for s in self._slots:
             if not s.busy and s.buf is not None:
-                if s.done_event is not None:
-                    s.done_event.synchronize()
+                s.wait_device_writes()
                 s.__dict__.pop("_exchange_views", None)
                 s.buf.close()
                 s.buf = None
@@ -1581,11 +1597,10 @@ class SnapshotEngine:
             plan.close()
         self._plans.clear()
         for s in self._slots:
-            if s.done_event is not None:
-                try:
-                    s.done_event.synchronize()
-                except SnapError:
-                    pass
+            try:
+                s.wait_device_writes()
+            except SnapError:
+                pass
             if s.buf is not None:
                 s.buf.close()
                 s.buf = None
