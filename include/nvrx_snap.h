@@ -34,7 +34,7 @@
 extern "C" {
 #endif
 
-#define NVRX_ABI_VERSION 5
+#define NVRX_ABI_VERSION 6
 
 enum {
     NVRX_OK = 0,
@@ -94,6 +94,12 @@ int nvrx_plan_layout(const nvrx_plan* plan, uint64_t* offsets, uint64_t* packed_
 /* Re-point the plan at a new set of tensors with identical sizes/flags (e.g. scatter destinations on
  * restore, or re-allocated parameters).  Alignment classes may change; the tile list is rebuilt. */
 int nvrx_plan_update_ptrs(nvrx_plan* plan, const void* const* ptrs);
+/* Re-point segments [seg_lo, seg_lo + n) at ptrs[0, n) while the snapshot ranges before them may still be in flight.  Only
+ * the changed entries are uploaded, from their own region of the pinned mirror, by the next upload (the next launch on the
+ * plan), which waits on the host only for an earlier upload of the same entries -- not for the disjoint ranges uploaded
+ * earlier in the same snapshot.  A pointer that changes its 16-byte alignment class would change the tile list:
+ * NVRX_E_STATE, nothing is changed, and the caller re-points the whole plan with nvrx_plan_update_ptrs instead. */
+int nvrx_plan_update_ptrs_range(nvrx_plan* plan, int64_t seg_lo, int64_t n, const void* const* ptrs);
 int nvrx_plan_set_variant(nvrx_plan* plan, int variant);
 /* Introspection (tests, tooling): the tile work-list a launch would walk -- tiles [0, *n_bulk) are the TMA-eligible ones,
  * the rest ragged; up to `capacity` entries are written to seg/nbytes/off (any may be NULL).  `shard_bytes` != 0 shows
@@ -148,8 +154,17 @@ int nvrx_drain(void* host_dst, const void* staging, uint64_t bytes, uint64_t chu
  * sub-launch -- the training stream is free from there; `done_event` (optional) on drain_stream after the last copy. */
 int nvrx_snapshot(nvrx_plan* plan, void* staging, void* host_dst, uint64_t chunk_bytes, volatile uint64_t* progress,
                   uint64_t base_value, void* pack_stream, void* drain_stream, void* packed_event, void* done_event);
-/* Kernel launches of the last nvrx_snapshot on this plan: the pack runs as a few sub-launches over geometrically growing
- * groups of copy chunks (1, 4, 16, ... chunks; NVRX_B200_PACK_GROWTH), 4 for a 16 GB snapshot with 256 MiB chunks. */
+/* nvrx_snapshot of the staging range of segments [seg_lo, seg_hi) alone: from off[seg_lo] (0 when seg_lo == 0) to
+ * off[seg_hi] (staging_bytes when seg_hi == n), cut into chunks and pack groups from the range's start by the same rule.
+ * Calls for consecutive ranges on the same streams make one snapshot whose first range can be launched while the tensors
+ * of the later ones are still being checked; nvrx_snapshot is the call for [0, n).  The progress word counts absolute
+ * staging bytes (base_value + end of each chunk), so it rises across the ranges. */
+int nvrx_snapshot_range(nvrx_plan* plan, int64_t seg_lo, int64_t seg_hi, void* staging, void* host_dst, uint64_t chunk_bytes,
+                        volatile uint64_t* progress, uint64_t base_value, void* pack_stream, void* drain_stream,
+                        void* packed_event, void* done_event);
+/* Kernel launches of the last snapshot on this plan: the pack runs as a few sub-launches over geometrically growing
+ * groups of copy chunks (1, 4, 16, ... chunks; NVRX_B200_PACK_GROWTH), 4 for a 16 GB snapshot with 256 MiB chunks.  A
+ * range starting at segment 0 sets the count, a later range adds its own. */
 int nvrx_plan_last_launches(const nvrx_plan* plan, uint32_t* launches);
 /* Mirror for restore: pinned host -> device staging (H2D), optional event. */
 int nvrx_fill(void* staging, const void* host_src, uint64_t bytes, uint64_t chunk_bytes, void* stream,

@@ -77,10 +77,14 @@ struct nvrx_plan {
     size_t segs_cap = 0, tiles_cap = 0;  // capacity (entries) of the pinned / device mirrors
     uint32_t n_bulk = 0, n_tiles = 0;
     bool segs_dirty = true, tiles_dirty = true;
+    // segment entries [range_lo, range_hi) re-pointed by nvrx_plan_update_ptrs_range and not uploaded yet
+    int64_t range_lo = 0, range_hi = 0;
+    // pinned segment entries [pend_lo, pend_hi) whose H2D may still be queued: rewriting them needs a host wait first
+    int64_t pend_lo = 0, pend_hi = 0;
     std::vector<cudaEvent_t> chunk_events;  // pack -> drain hand-off of the pipelined snapshot
     cudaEvent_t upload_done = nullptr;      // last H2D of the descriptor mirrors (they are reused)
     cudaEvent_t last_launch = nullptr;      // last kernel launch that reads the device mirrors, on whichever stream it ran
-    uint32_t last_launches = 0;             // kernel launches of the last nvrx_snapshot (its pack groups)
+    uint32_t last_launches = 0;             // pack launches of the last snapshot (summed over its ranges)
 };
 
 namespace {
@@ -207,15 +211,40 @@ void fill_segs(nvrx_plan* p) {
     p->segs_dirty = true;
 }
 
+// Upload of the segment entries [range_lo, range_hi) alone, from their own region of the pinned mirror.  The host waits for
+// an earlier upload only when that upload covered part of this region (the previous snapshot's, typically), never for the
+// disjoint ranges uploaded earlier in the same snapshot, so the ranges of one snapshot do not serialise on the host.
+int upload_range(nvrx_plan* p, cudaStream_t st) {
+    const int64_t lo = p->range_lo, hi = p->range_hi;
+    p->range_lo = p->range_hi = 0;
+    if (lo < p->pend_hi && p->pend_lo < hi) {
+        NVRX_CUDA(cudaEventSynchronize(p->upload_done));
+        p->pend_lo = p->pend_hi = 0;
+    }
+    // the device entries are about to be rewritten: a launch queued earlier on another stream must have read them first
+    if (p->last_launch) NVRX_CUDA(cudaStreamWaitEvent(st, p->last_launch, 0));
+    const size_t n = static_cast<size_t>(hi - lo);
+    memcpy(p->pin_segs + lo, p->h_segs.data() + lo, n * sizeof(SegDesc));
+    NVRX_CUDA(cudaMemcpyAsync(p->d_segs + lo, p->pin_segs + lo, n * sizeof(SegDesc), cudaMemcpyHostToDevice, st));
+    NVRX_CUDA(cudaEventRecord(p->upload_done, st));
+    p->pend_lo = p->pend_lo < p->pend_hi ? std::min(p->pend_lo, lo) : lo;
+    p->pend_hi = std::max(p->pend_hi, hi);
+    return NVRX_OK;
+}
+
 int upload(nvrx_plan* p, cudaStream_t st) {
     if (p->sm_count == 0) NVRX_CUDA(cudaDeviceGetAttribute(&p->sm_count, cudaDevAttrMultiProcessorCount, p->device));
     if (!(p->segs_dirty && p->n > 0) && !(p->tiles_dirty && p->n_tiles > 0)) {
         p->segs_dirty = p->tiles_dirty = false;
-        return NVRX_OK;
+        // entries re-pointed range by range go alone (the mirrors exist: the whole table was uploaded before)
+        return p->range_lo < p->range_hi ? upload_range(p, st) : NVRX_OK;
     }
+    if (p->range_lo < p->range_hi) p->segs_dirty = true;  // re-pointed entries travel with the whole table
+    p->range_lo = p->range_hi = 0;
     // the pinned mirrors are about to be rewritten: an earlier upload must have finished reading them
     if (p->upload_done) NVRX_CUDA(cudaEventSynchronize(p->upload_done));
     else NVRX_CUDA(cudaEventCreateWithFlags(&p->upload_done, cudaEventDisableTiming));
+    p->pend_lo = p->pend_hi = 0;
     // the device mirrors are about to be rewritten or freed: a launch queued earlier, possibly on another stream (a cached
     // plan re-pointed with update_ptrs and launched on a new stream), must have read them first.  The H2D waits on the
     // device; only freeing them for a larger table waits on the host.
@@ -236,6 +265,7 @@ int upload(nvrx_plan* p, cudaStream_t st) {
         }
         memcpy(p->pin_segs, p->h_segs.data(), n * sizeof(SegDesc));
         NVRX_CUDA(cudaMemcpyAsync(p->d_segs, p->pin_segs, n * sizeof(SegDesc), cudaMemcpyHostToDevice, st));
+        p->pend_hi = p->n;
     }
     p->segs_dirty = false;
     if (p->tiles_dirty && p->n_tiles > 0) {
@@ -512,6 +542,33 @@ int nvrx_plan_update_ptrs(nvrx_plan* p, const void* const* ptrs) {
     return NVRX_OK;
 }
 
+int nvrx_plan_update_ptrs_range(nvrx_plan* p, int64_t seg_lo, int64_t n, const void* const* ptrs) {
+    if (!p || seg_lo < 0 || n < 0 || seg_lo > p->n - n || (n > 0 && !ptrs)) return NVRX_E_INVALID;
+    int64_t first = -1, last = -1;
+    for (int64_t k = 0; k < n; ++k) {
+        const int64_t i = seg_lo + k;
+        const uint64_t np = reinterpret_cast<uint64_t>(ptrs[k]);
+        if (p->nbytes[i] && !np) return NVRX_E_INVALID;
+        if ((p->flags[i] & NVRX_SEG_NARROW_F32_BF16) && (np & 3u)) return NVRX_E_INVALID;
+        if (((np ^ p->ptrs[i]) & 15u) != 0) return NVRX_E_STATE;  // the tile list changes: nvrx_plan_update_ptrs
+        if (np != p->ptrs[i]) {
+            if (first < 0) first = i;
+            last = i;
+        }
+    }
+    if (first < 0) return NVRX_OK;
+    for (int64_t i = first; i <= last; ++i) {
+        p->ptrs[i] = reinterpret_cast<uint64_t>(ptrs[i - seg_lo]);
+        p->h_segs[i].ptr = p->ptrs[i];
+    }
+    if (!p->segs_dirty) {  // otherwise the whole table goes up with the next upload anyway
+        const bool empty = p->range_lo >= p->range_hi;
+        p->range_lo = empty ? first : std::min(p->range_lo, first);
+        p->range_hi = empty ? last + 1 : std::max(p->range_hi, last + 1);
+    }
+    return NVRX_OK;
+}
+
 int nvrx_plan_set_shard_rotation(nvrx_plan* p, uint32_t first_shard) {
     if (!p) return NVRX_E_INVALID;
     if (p->first_shard != first_shard) {
@@ -627,8 +684,17 @@ int nvrx_pack_sharded(nvrx_plan* p, void* staging, void* const* peer_bases, int 
 
 int nvrx_snapshot(nvrx_plan* p, void* staging, void* host_dst, uint64_t chunk_bytes, volatile uint64_t* progress,
                   uint64_t base_value, void* pack_stream, void* drain_stream, void* packed_event, void* done_event) {
+    if (!p) return NVRX_E_INVALID;
+    return nvrx_snapshot_range(p, 0, p->n, staging, host_dst, chunk_bytes, progress, base_value, pack_stream, drain_stream,
+                               packed_event, done_event);
+}
+
+int nvrx_snapshot_range(nvrx_plan* p, int64_t seg_lo, int64_t seg_hi, void* staging, void* host_dst, uint64_t chunk_bytes,
+                        volatile uint64_t* progress, uint64_t base_value, void* pack_stream, void* drain_stream,
+                        void* packed_event, void* done_event) {
     if (!p || (p->staging_bytes && (!staging || !host_dst))) return NVRX_E_INVALID;
     if (reinterpret_cast<uintptr_t>(staging) & 511u) return NVRX_E_INVALID;
+    if (seg_lo < 0 || seg_lo > seg_hi || seg_hi > p->n) return NVRX_E_INVALID;
     DeviceGuard guard(p->device);
     if (p->shard_bytes) {
         p->shard_bytes = 0;
@@ -638,7 +704,13 @@ int nvrx_snapshot(nvrx_plan* p, void* staging, void* host_dst, uint64_t chunk_by
     cudaStream_t ps = static_cast<cudaStream_t>(pack_stream), ds = static_cast<cudaStream_t>(drain_stream);
     int rc = upload(p, ps);
     if (rc) return rc;
-    const uint64_t total = p->staging_bytes;
+    // the staging range of the segments: from the first one's offset (0 for the first range, so that the ranges of a
+    // snapshot tile the whole staging buffer) to the next segment's offset (the end of staging for the last range)
+    const uint64_t first = seg_lo == 0 ? 0 : p->off[seg_lo];
+    const uint64_t last = seg_hi == p->n ? p->staging_bytes : p->off[seg_hi];
+    const uint64_t total = last - first;
+    uint8_t* const stg = static_cast<uint8_t*>(staging) + first;
+    uint8_t* const dst = static_cast<uint8_t*>(host_dst) + first;
     if (chunk_bytes == 0 || chunk_bytes > total) chunk_bytes = total ? total : 1;
     chunk_bytes = round_up(chunk_bytes, 512);
     uint64_t n_chunks = total ? (total + chunk_bytes - 1) / chunk_bytes : 0;
@@ -662,15 +734,19 @@ int nvrx_snapshot(nvrx_plan* p, void* staging, void* host_dst, uint64_t chunk_by
     // stay `chunk_bytes` long (granularity of the progress word the writer follows).
     uint64_t growth = 4;
     if (const char* env = getenv("NVRX_B200_PACK_GROWTH")) growth = std::max<long long>(1, atoll(env));
-    uint32_t b_lo = 0, r_lo = p->n_bulk;
+    // the range's tiles: bulk [b_lo, b_end), ragged [r_lo, r_end) (both lists are sorted by staging position)
+    const bool to_end = seg_hi == p->n;
+    uint32_t b_lo = lower_tile(p, 0, p->n_bulk, first), r_lo = lower_tile(p, p->n_bulk, p->n_tiles, first);
+    const uint32_t b_end = to_end ? p->n_bulk : lower_tile(p, b_lo, p->n_bulk, last);
+    const uint32_t r_end = to_end ? p->n_tiles : lower_tile(p, r_lo, p->n_tiles, last);
     uint64_t c = 0, group = 1, n_groups = 0;
     while (c < n_chunks) {
         const uint64_t g_end = std::min(n_chunks, c + group);
-        const uint64_t end_pos = std::min(total, g_end * chunk_bytes);
+        const uint64_t end_pos = first + std::min(total, g_end * chunk_bytes);
         // group = every tile that STARTS before end_pos and was not launched yet; a tile reaching into the next group
         // is complete before that group's event, which is what that group's copies wait for
-        const uint32_t b_hi = (g_end == n_chunks) ? p->n_bulk : lower_tile(p, b_lo, p->n_bulk, end_pos);
-        const uint32_t r_hi = (g_end == n_chunks) ? p->n_tiles : lower_tile(p, r_lo, p->n_tiles, end_pos);
+        const uint32_t b_hi = (g_end == n_chunks) ? b_end : lower_tile(p, b_lo, b_end, end_pos);
+        const uint32_t r_hi = (g_end == n_chunks) ? r_end : lower_tile(p, r_lo, r_end, end_pos);
         TileSpan span;
         span.a = p->d_tiles + b_lo;
         span.na = b_hi - b_lo;
@@ -685,18 +761,18 @@ int nvrx_snapshot(nvrx_plan* p, void* staging, void* host_dst, uint64_t chunk_by
         ++n_groups;
         for (; c < g_end; ++c) {
             const uint64_t begin = c * chunk_bytes, stop = std::min(total, (c + 1) * chunk_bytes);
-            NVRX_CUDA(cudaMemcpyAsync(static_cast<uint8_t*>(host_dst) + begin, static_cast<const uint8_t*>(staging) + begin,
-                                      stop - begin, cudaMemcpyDeviceToHost, ds));
-            if (prog_dev) {
-                rc = nvrx_stream_write_u64(ds, prog_dev, base_value + stop);
+            NVRX_CUDA(cudaMemcpyAsync(dst + begin, stg + begin, stop - begin, cudaMemcpyDeviceToHost, ds));
+            if (prog_dev) {  // absolute staging bytes: the word keeps rising across the ranges of a snapshot
+                rc = nvrx_stream_write_u64(ds, prog_dev, base_value + first + stop);
                 if (rc) return rc;
             }
         }
         group *= growth;
     }
-    p->last_launches = static_cast<uint32_t>(n_groups);
+    // the first range of a snapshot starts the count, later ones add theirs
+    p->last_launches = static_cast<uint32_t>(n_groups) + (seg_lo == 0 ? 0 : p->last_launches);
     if (n_chunks == 0 && prog_dev) {
-        rc = nvrx_stream_write_u64(ds, prog_dev, base_value);
+        rc = nvrx_stream_write_u64(ds, prog_dev, base_value + last);
         if (rc) return rc;
     }
     if (packed_event) NVRX_CUDA(cudaEventRecord(static_cast<cudaEvent_t>(packed_event), ps));

@@ -7,12 +7,13 @@ and one side-stream drain, and the request carries only a snapshot descriptor; t
 the drain on the shared progress word and then runs ``torch.save`` on views of the pinned slot.
 """
 
+import itertools
 import logging
 
 import torch
 
 from ..b200.persist import SnapshotRef, save_snapshot_with_torch
-from ..utils import _collect_tensors, dict_list_map_outplace, preload_tensors, wrap_for_async
+from ..utils import _collect_tensors, _walk_tensors, dict_list_map_outplace, preload_tensors, wrap_for_async
 from .core import AsyncCallsQueue, AsyncRequest
 
 logger = logging.getLogger(__name__)
@@ -34,10 +35,11 @@ class TorchAsyncCheckpoint(object):
         """Same calling convention as ``torch.save(state_dict, f, ...)``; returns once the snapshot is
         *enqueued* on the GPU (pack kernel on the current stream, drain on a side stream)."""
         self._reap()
-        tensors = []
-        _collect_tensors(state_dict, tensors)
-        cuda = [t for t in tensors if t.is_cuda]
-        if not cuda:
+        # a lazy walk: the engine checks each tensor as it comes and launches the pack of a staging range as soon as all of
+        # its tensors passed, so walking and checking the rest of the state runs beside the GPU's work
+        cuda = (t for t in _walk_tensors(state_dict) if t.is_cuda)
+        first = next(cuda, None)
+        if first is None:
             # nothing on the GPU (reference config C1): the host tensors go to the writer as they are
             request = AsyncRequest(TorchAsyncCheckpoint.async_fn, (preload_tensors(state_dict), *args), [], kwargs or {})
             self._async_calls_queue.schedule_async_request(request)
@@ -48,8 +50,8 @@ class TorchAsyncCheckpoint(object):
         # same dict (e.g. ``torch.get_rng_state()``) travel to the writer as they are, like in the reference, whose
         # ``preload_tensors`` maps them through ``.to("cpu")`` = identity (``utils.py:93-94``).
         # (the engine checks that all of them live on ONE device and raises ValueError otherwise)
-        snap = SnapshotEngine.get(cuda[0].get_device()).snapshot(cuda, narrow=self._narrow)
-        counter = iter(range(len(cuda)))
+        snap = SnapshotEngine.get(first.get_device()).snapshot(itertools.chain((first,), cuda), narrow=self._narrow)
+        counter = iter(range(snap.n_total))
 
         def leaf(v):
             if isinstance(v, torch.Tensor):

@@ -12,7 +12,7 @@ import os
 from pathlib import Path
 from typing import Optional
 
-ABI_VERSION = 5
+ABI_VERSION = 6
 
 OK = 0
 E_INVALID = 1000
@@ -47,6 +47,7 @@ EXPORTED_SYMBOLS = (
     "nvrx_plan_info",
     "nvrx_plan_layout",
     "nvrx_plan_update_ptrs",
+    "nvrx_plan_update_ptrs_range",
     "nvrx_plan_set_variant",
     "nvrx_plan_tiles",
     "nvrx_plan_commit",
@@ -57,6 +58,7 @@ EXPORTED_SYMBOLS = (
     "nvrx_pack_broadcast",
     "nvrx_drain",
     "nvrx_snapshot",
+    "nvrx_snapshot_range",
     "nvrx_plan_last_launches",
     "nvrx_fill",
     "nvrx_fill_from_fd",
@@ -158,6 +160,7 @@ def _declare(lib: C.CDLL) -> None:
         "nvrx_plan_info": (_int, [_vp, P(_u64), P(_u64), P(_u64)]),
         "nvrx_plan_layout": (_int, [_vp, P(_u64), P(_u64)]),
         "nvrx_plan_update_ptrs": (_int, [_vp, P(_vp)]),
+        "nvrx_plan_update_ptrs_range": (_int, [_vp, _i64, _i64, P(_vp)]),
         "nvrx_plan_set_variant": (_int, [_vp, _int]),
         "nvrx_plan_tiles": (_int, [_vp, _u64, P(_u32), P(_u32), P(_u32), P(_u32), P(_u64), _u64]),
         "nvrx_plan_commit": (_int, [_vp, _vp]),
@@ -168,6 +171,7 @@ def _declare(lib: C.CDLL) -> None:
         "nvrx_pack_broadcast": (_int, [_vp, P(_vp), _int, _u64, _vp]),
         "nvrx_drain": (_int, [_vp, _vp, _u64, _u64, _vp, _u64, _vp, _vp]),
         "nvrx_snapshot": (_int, [_vp, _vp, _vp, _u64, _vp, _u64, _vp, _vp, _vp, _vp]),
+        "nvrx_snapshot_range": (_int, [_vp, _i64, _i64, _vp, _vp, _u64, _vp, _u64, _vp, _vp, _vp, _vp]),
         "nvrx_plan_last_launches": (_int, [_vp, P(_u32)]),
         "nvrx_fill": (_int, [_vp, _vp, _u64, _u64, _vp, _vp]),
         "nvrx_fill_from_fd": (_int, [_vp, _u64, _int, _i64, P(_u64), P(_u64), P(_u64), _u64, _int, _int, _int, _vp]),

@@ -20,14 +20,16 @@ There is no CPU fallback: everything here raises if ``libnvrx_snap.so`` or a CUD
 
 from __future__ import annotations
 
+import bisect
 import ctypes as C
 import logging
 import os
 import re
 import threading
+import time
 import uuid
 from dataclasses import dataclass, field
-from typing import Dict, List, NamedTuple, Optional, Sequence, Tuple
+from typing import Dict, Iterable, Iterator, List, NamedTuple, Optional, Sequence, Tuple
 
 import torch
 
@@ -91,7 +93,8 @@ class Plan:
         check(self._lib.nvrx_plan_layout(self._h, offs, packed), "nvrx_plan_layout")
         self.offsets: Tuple[int, ...] = tuple(offs[i] for i in range(self.n))
         self.packed_nbytes: Tuple[int, ...] = tuple(packed[i] for i in range(self.n))
-        self.ptrs: Tuple[int, ...] = tuple(ptrs)
+        self.nbytes: Tuple[int, ...] = tuple(nbytes)
+        self.ptrs: List[int] = list(ptrs)
         if variant != _cabi.VARIANT_AUTO:
             self.set_variant(variant)
 
@@ -120,10 +123,25 @@ class Plan:
 
     def update_ptrs(self, ptrs: Sequence[int]) -> None:
         assert len(ptrs) == self.n
-        if tuple(ptrs) == self.ptrs:
+        ptrs = list(ptrs)
+        if ptrs == self.ptrs:
             return
         check(self._lib.nvrx_plan_update_ptrs(self._h, _ptr_array(ptrs)), "nvrx_plan_update_ptrs")
-        self.ptrs = tuple(ptrs)
+        self.ptrs = ptrs
+
+    def update_ptrs_range(self, lo: int, ptrs: List[int]) -> bool:
+        """Re-point segments ``[lo, lo + len(ptrs))`` (``nvrx_plan_update_ptrs_range``) while earlier ranges of a snapshot may
+        still be packing.  False, and nothing changed, when a pointer moved to another 16-byte alignment class: the tile
+        list would change, which only :meth:`update_ptrs` does."""
+        hi = lo + len(ptrs)
+        if ptrs == self.ptrs[lo:hi]:
+            return True
+        rc = self._lib.nvrx_plan_update_ptrs_range(self._h, lo, len(ptrs), _ptr_array(ptrs))
+        if rc == _cabi.E_STATE:
+            return False
+        check(rc, "nvrx_plan_update_ptrs_range")
+        self.ptrs[lo:hi] = ptrs
+        return True
 
     def commit(self, stream: int) -> None:
         check(self._lib.nvrx_plan_commit(self._h, stream), "nvrx_plan_commit")
@@ -756,6 +774,30 @@ class Snapshot:
             self.engine._release(self.slot)
 
 
+# pack groups of one nvrx_snapshot call cover 1, 4, 16, ... drain chunks (NVRX_B200_PACK_GROWTH's default)
+_RANGE_GROWTH = 4
+
+
+def staging_ranges(offsets: Sequence[int], staging_bytes: int, chunk: int) -> List[int]:
+    """Segment bounds ``[0, s_1, ..., n]`` of the ranges a staged snapshot launches one after the other.  They follow the pack
+    groups of a whole-snapshot call: range k ends at the first segment whose offset reaches the end of group k (256 MiB,
+    1.25 GiB, 5.25 GiB, ... with 256 MiB chunks) and the last range runs to the end.  The first range is small, so the GPU
+    starts after a few checks; every later one is about four times its predecessor, so its checks fit beside that pack."""
+    bounds, end, group = [0], 0, 1
+    while True:
+        end += group * chunk
+        group *= _RANGE_GROWTH
+        if end >= staging_bytes:
+            break
+        i = bisect.bisect_left(offsets, end)
+        if i >= len(offsets):
+            break
+        if i > bounds[-1]:
+            bounds.append(i)
+    bounds.append(len(offsets))
+    return bounds
+
+
 def choose_slot(slots: Sequence[_Slot], nbytes: int, max_slots: int) -> Tuple[Optional[_Slot], bool]:
     """Which slot the next snapshot of ``nbytes`` goes to: ``(slot, retire)``.
 
@@ -859,6 +901,8 @@ class SnapshotEngine:
             if stale:
                 logger.warning(f"removed {len(stale)} snapshot slot(s) left behind by dead processes: {stale[:4]}...")
         self._plans: Dict[tuple, Plan] = {}
+        # narrow -> (nbytes, narrowing mask or None) of the last snapshot that a staged snapshot could repeat
+        self._last_structure: Dict[bool, Tuple[Tuple[int, ...], Optional[Tuple[bool, ...]]]] = {}
         self._staging: Optional[DeviceBuffer] = None
         self._staging_free: Optional[Event] = None  # recorded when the last reader of staging finished
         self._side = Stream(self.device)
@@ -973,6 +1017,15 @@ class SnapshotEngine:
                 self._release(s)
 
     # ---- planning -------------------------------------------------------------------------------
+    @staticmethod
+    def _plan_key(nbytes: Sequence[int], narrow: Optional[Sequence[bool]], container: bool,
+                  offsets: Optional[Sequence[int]] = None) -> tuple:
+        # a bit copy does not care about dtypes (the layout handed to readers does: it is validated where it is cached)
+        key = (tuple(nbytes), tuple(narrow) if narrow is not None else None)
+        if offsets is not None:
+            return ("at", tuple(offsets)) + key
+        return ("container",) + key if container else key
+
     def _plan_for(
         self, tensors: Sequence[torch.Tensor], narrow: Sequence[bool], container: bool = False,
         offsets: Optional[Sequence[int]] = None,
@@ -984,12 +1037,7 @@ class SnapshotEngine:
         nbytes = [t.nbytes for t in tensors]
         if narrow is not None and not any(narrow):
             narrow = None
-        # a bit copy does not care about dtypes (the layout handed to readers does: it is validated where it is cached)
-        key = (tuple(nbytes), tuple(narrow) if narrow is not None else None)
-        if offsets is not None:
-            key = ("at", tuple(offsets)) + key
-        elif container:
-            key = ("container",) + key
+        key = self._plan_key(nbytes, narrow, container, offsets)
         ptrs = [t.data_ptr() if nb else 0 for t, nb in zip(tensors, nbytes)]
         plan = self._plans.get(key)
         if plan is None:
@@ -1013,19 +1061,137 @@ class SnapshotEngine:
     def _narrow_mask(tensors: Sequence[torch.Tensor], narrow: bool) -> List[bool]:
         return [bool(narrow) and t.dtype == torch.float32 and t.numel() > 0 for t in tensors]
 
+    def _staged_plan(self, narrow: bool, container: bool) -> Optional[Tuple[Plan, bool]]:
+        """``(plan, container)`` for a staged snapshot: the cached plan of the last structure snapshotted with this ``narrow``,
+        when it spans more than one drain chunk (a snapshot of one chunk has nothing to overlap its checks with)."""
+        last = self._last_structure.get(bool(narrow))
+        if last is None or self.timing:
+            return None
+        container = bool(container) and self._spare_slots() > 1  # the rule of _snapshot_all for a list without passthrough
+        plan = self._plans.get(self._plan_key(last[0], last[1], container))
+        if plan is None or plan.staging_bytes <= self.drain_chunk:
+            return None
+        return plan, container
+
     # ---- snapshot -------------------------------------------------------------------------------
-    def snapshot(self, tensors: Sequence[torch.Tensor], *, narrow: bool = False, container: Optional[bool] = None) -> Snapshot:
+    def snapshot(self, tensors: Iterable[torch.Tensor], *, narrow: bool = False, container: Optional[bool] = None) -> Snapshot:
         """Pack ``tensors`` (CUDA tensors of this device; others pass through) and start the drain.
 
         Returns as soon as the pack kernel and the side-stream copy are *enqueued*.  ``container`` (default: the
-        ``NVRX_B200_ZERO_COPY`` switch) packs in checkpoint-container geometry, see :meth:`_plan_for`."""
+        ``NVRX_B200_ZERO_COPY`` switch) packs in checkpoint-container geometry, see :meth:`_plan_for`.  ``tensors`` may be
+        a lazy walk: when it has the structure of the previous snapshot, the first staging range is launched as soon as its
+        tensors are checked, and the later ranges are checked while it packs (:meth:`_snapshot_staged`)."""
         trace = self.trace
         if trace is not None:
-            import time as _time
-
             trace.clear()
-            trace["enter"] = _time.perf_counter()
-        all_tensors = tensors if isinstance(tensors, list) else list(tensors)
+            trace["enter"] = time.perf_counter()
+        if container is None:
+            from .fastsave import zero_copy_enabled
+
+            container = zero_copy_enabled()
+        staged = self._staged_plan(narrow, container)
+        if staged is not None:
+            return self._snapshot_staged(staged[0], staged[1], iter(tensors), narrow, container)
+        return self._snapshot_all(tensors if isinstance(tensors, list) else list(tensors), narrow, container)
+
+    def _snapshot_staged(self, plan: Plan, container: bool, it: Iterator[torch.Tensor], narrow: bool, requested: bool) -> Snapshot:
+        """Snapshot of the structure ``plan`` was made for, launched range by range (:func:`staging_ranges`) while ``it`` is
+        walked.  Every tensor is checked against its segment (device, contiguity, size, narrowing); a range is re-pointed and
+        launched once its last tensor passed, so the checks of the later ranges run while the earlier ones pack, and no
+        kernel reads a pointer that was not checked in this call.
+
+        A tensor that fails its check, or another tensor count, ends the staging: the walk is finished and the whole list
+        goes through :meth:`_snapshot_all` into the same slot.  Launched ranges only wrote checked bytes into staging and the
+        slot; the full snapshot's pack waits for their drain and its progress values start behind what they drained."""
+        trace = self.trace
+        cached = plan.__dict__.get("_ranges")
+        if cached is None or cached[0] != self.drain_chunk:
+            cached = plan.__dict__["_ranges"] = (self.drain_chunk, staging_ranges(plan.offsets, plan.staging_bytes, self.drain_chunk))
+        bounds = cached[1]
+        stream = self._current_stream()
+        staging = self._ensure_staging(plan.staging_bytes)
+        crc, need, crc_off, ready_off = self._crc_room(plan)
+        tail_room = 0
+        if container:
+            from .ptzip import slot_tail_room
+
+            tail_room = slot_tail_room(plan.n)
+        slot = self._acquire_slot(need + tail_room)
+        if self._staging_free is not None:
+            stream_wait_event(stream, self._staging_free)
+        packed_ev = Event(self.device) if crc is not None else None
+        base = slot.drained_total
+        dev, nbytes, f32 = self.device, plan.nbytes, torch.float32
+        want = self._last_structure[bool(narrow)][1] if narrow else None
+        if narrow and want is None:
+            want = (False,) * plan.n
+        seen: List[torch.Tensor] = []
+        lo = 0
+        ok = True
+        for hi in bounds[1:]:
+            ptrs = []
+            for j in range(lo, hi):
+                t = next(it, None)
+                if t is None:
+                    ok = False
+                    break
+                seen.append(t)
+                nb = t.nbytes
+                if (nb != nbytes[j] or t.get_device() != dev or not t.is_contiguous()
+                        or (want is not None and want[j] != (nb > 0 and t.dtype == f32))):
+                    ok = False
+                    break
+                ptrs.append(t.data_ptr() if nb else 0)
+            if not ok or not plan.update_ptrs_range(lo, ptrs):
+                ok = False
+                break
+            if trace is not None and lo == 0:
+                trace["planned"] = time.perf_counter()
+            check(
+                self.lib.nvrx_snapshot_range(
+                    plan._h, lo, hi, staging.ptr, slot.buf.data_ptr, self.drain_chunk, slot.buf.progress_ptr, base, stream,
+                    self._side.handle, packed_ev.handle if packed_ev is not None else None, slot.done_event.handle,
+                ),
+                "nvrx_snapshot_range",
+            )
+            lo = hi
+        if ok:
+            extra = next(it, None)
+            if extra is not None:
+                seen.append(extra)
+                ok = False
+        if not ok:
+            seen.extend(it)
+            if lo:
+                self.launches += plan.last_launches()
+                slot.drained_total = base + (plan.offsets[lo] if lo < plan.n else plan.staging_bytes)
+                self._staging_free = slot.done_event  # the full pack rewrites staging the launched copies may still read
+            return self._snapshot_all(seen, narrow, requested, slot=slot)
+        if trace is not None:
+            trace["launched"] = time.perf_counter()
+        self.launches += plan.last_launches() if plan.n_tiles else 0
+        slot.drained_total = base + plan.staging_bytes
+        self._staging_free = slot.done_event
+        mask = list(want) if want is not None and any(want) else None
+        return self._finish_snapshot(plan, slot, staging, crc, crc_off, ready_off, packed_ev, seen, mask, {}, len(seen))
+
+    def _crc_room(self, plan: Plan):
+        """``(crc plan or None, slot bytes needed, offset of the checksum values, offset of the ready word)``: with GPU
+        checksums the values and the ready word sit behind the payload in the slot."""
+        if not gpu_crc_enabled() or plan.n == 0:
+            return None, plan.staging_bytes, 0, 0
+        crc = getattr(plan, "_crc", None)
+        if crc is None:
+            crc = plan._crc = CrcPlan(plan.offsets, plan.packed_nbytes, self.device)
+        crc_off = -(-plan.staging_bytes // 64) * 64  # partial values, then the ready word, behind the payload
+        ready_off = crc_off + -(-4 * crc.n_values // 8) * 8
+        return crc, ready_off + 8, crc_off, ready_off
+
+    def _snapshot_all(self, all_tensors: List[torch.Tensor], narrow: bool, container: bool,
+                      slot: Optional[_Slot] = None) -> Snapshot:
+        """Snapshot of the whole list in one ``nvrx_snapshot`` call, whatever its structure (``slot``: the one a staged
+        snapshot that gave up already holds)."""
+        trace = self.trace
         dev = self.device
         # everything up to the launch is on the training stream's critical path (the stall): one cheap test for the common
         # case (all tensors on this device, contiguous), the general bookkeeping only when it fails
@@ -1034,25 +1200,29 @@ class SnapshotEngine:
         if not all([t.get_device() == dev for t in all_tensors]):
             passthrough = {i: t for i, t in enumerate(all_tensors) if t.get_device() != dev}
             if any(t.is_cuda for t in passthrough.values()):
+                if slot is not None:
+                    self._release(slot)
                 raise ValueError("snapshot: the CUDA tensors must live on one device (the engine's)")
             cuda_tensors = [t for i, t in enumerate(all_tensors) if i not in passthrough]
         # the kernel walks contiguous byte ranges; strided tensors are compacted first (rare)
-        if not all([t.is_contiguous() for t in cuda_tensors]):
+        compacted = not all([t.is_contiguous() for t in cuda_tensors])
+        if compacted:
             cuda_tensors = [t if t.is_contiguous() else t.detach().contiguous() for t in cuda_tensors]
         mask = self._narrow_mask(cuda_tensors, narrow) if narrow else None
-        if container is None:
-            from .fastsave import zero_copy_enabled
-
-            container = zero_copy_enabled()
         container = bool(container) and not passthrough and len(cuda_tensors) > 0
         if container and self._spare_slots() <= 1:
             # every published checkpoint pins one slot until its file is deleted.  Keep the last slot that is not somebody's
             # checkpoint for copying saves, instead of publishing it too and paying a 16 GB re-pin on the next save
             container = False
         plan = self._plan_for(cuda_tensors, mask, container)
+        # the next snapshot of this structure may be staged (only one its checks can pass: on this device, contiguous)
+        if passthrough or compacted or not cuda_tensors:
+            self._last_structure.pop(bool(narrow), None)
+        else:
+            self._last_structure[bool(narrow)] = (plan.nbytes, tuple(mask) if mask is not None and any(mask) else None)
 
         if trace is not None:
-            trace["planned"] = _time.perf_counter()
+            trace["planned"] = time.perf_counter()
         stream = self._current_stream()
         staging = self._ensure_staging(plan.staging_bytes)
         tail_room = 0
@@ -1060,16 +1230,8 @@ class SnapshotEngine:
             from .ptzip import slot_tail_room
 
             tail_room = slot_tail_room(len(cuda_tensors))
-        crc = None
-        need = plan.staging_bytes
-        if gpu_crc_enabled() and not passthrough and len(cuda_tensors) > 0:
-            crc = getattr(plan, "_crc", None)
-            if crc is None:
-                crc = plan._crc = CrcPlan(plan.offsets, plan.packed_nbytes, self.device)
-            crc_off = -(-plan.staging_bytes // 64) * 64  # partial values, then the ready word, behind the payload
-            ready_off = crc_off + -(-4 * crc.n_values // 8) * 8
-            need = ready_off + 8
-        slot = self._acquire_slot(need + tail_room)
+        crc, need, crc_off, ready_off = self._crc_room(plan) if not passthrough else (None, plan.staging_bytes, 0, 0)
+        slot = self._acquire_slot(need + tail_room, slot)
         if self._staging_free is not None:
             # the previous drain may still be reading staging: order the pack after it on the GPU
             stream_wait_event(stream, self._staging_free)
@@ -1104,10 +1266,16 @@ class SnapshotEngine:
                 "nvrx_snapshot",
             )
         if trace is not None:
-            trace["launched"] = _time.perf_counter()
+            trace["launched"] = time.perf_counter()
         self.launches += (plan.last_launches() if not self.timing else 1) if plan.n_tiles else 0
         slot.drained_total = base + plan.staging_bytes
         self._staging_free = slot.done_event
+        return self._finish_snapshot(plan, slot, staging, crc, crc_off, ready_off, packed_ev, cuda_tensors, mask, passthrough,
+                                     len(all_tensors), start, stop)
+
+    def _finish_snapshot(self, plan, slot, staging, crc, crc_off, ready_off, packed_ev, cuda_tensors, mask, passthrough,
+                         n_total, start=None, stop=None) -> Snapshot:
+        """Bookkeeping once every pack launch is enqueued (it runs while they execute): the checksum kernel, the layout."""
         crc_info = None
         if crc is not None:
             # checksum kernel on a third stream, concurrent with the drain: reads staging once more, sends one 32-bit value per
@@ -1147,7 +1315,7 @@ class SnapshotEngine:
             plan.__dict__["_layout"] = (shapes, layout, dtypes)
         return Snapshot(
             engine=self, slot=slot, layout=layout, progress_target=slot.drained_total, passthrough=passthrough,
-            n_total=len(all_tensors), pack_start=start, pack_stop=stop, crc_info=crc_info,
+            n_total=n_total, pack_start=start, pack_stop=stop, crc_info=crc_info,
         )
 
     # ---- restore --------------------------------------------------------------------------------

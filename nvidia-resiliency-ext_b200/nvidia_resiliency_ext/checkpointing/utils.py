@@ -95,6 +95,23 @@ def _collect_tensors(x, out: list) -> None:
         out.append(x)
 
 
+def _walk_tensors(x):
+    """The tensors of ``x`` in ``_collect_tensors`` order (depth first through dicts and lists), yielded one at a time."""
+    stack = [iter((x,))]
+    while stack:
+        for v in stack[-1]:
+            if isinstance(v, torch.Tensor):
+                yield v
+            elif isinstance(v, dict):
+                stack.append(iter(v.values()))
+                break
+            elif isinstance(v, list):
+                stack.append(iter(v))
+                break
+        else:
+            stack.pop()
+
+
 def preload_tensors(state_dict: Dict, non_blocking=True, *, narrow: bool = False, return_snapshot: bool = False):
     """Stage every tensor of ``state_dict`` in host memory; returns a new dict with CPU tensors.
 
