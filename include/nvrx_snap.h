@@ -34,7 +34,7 @@
 extern "C" {
 #endif
 
-#define NVRX_ABI_VERSION 6
+#define NVRX_ABI_VERSION 7
 
 enum {
     NVRX_OK = 0,
@@ -137,6 +137,13 @@ int nvrx_plan_set_shard_rotation(nvrx_plan* plan, uint32_t first_shard);
  * HBM once; remote copies travel as NVLink P2P stores issued by the same kernel (TMA bulk stores from the one
  * shared-memory slot, or STG.128 on the ragged path).  Callers order it between two clique barriers. */
 int nvrx_pack_broadcast(nvrx_plan* plan, void* const* peer_bases, int n_peers, uint64_t slot_offset, void* stream);
+
+/* ---- parity of erasure-coded local checkpoints ---------------------------------------------------
+ * dst[0, bytes) = srcs[0] ^ srcs[1] ^ ... ^ srcs[n-1] over [0, bytes); with clear_srcs != 0 every source range is zero
+ * afterwards.  One launch on `stream` (on the current device).  Device pointers 16-byte aligned, bytes % 16 == 0,
+ * 1 <= n <= 64, dst must not overlap any source; otherwise NVRX_E_INVALID.  bytes may exceed 2^32; bytes == 0 launches
+ * nothing.  Algorithmic HBM bytes: (n + 1) * bytes, (2n + 1) * bytes with clearing. */
+int nvrx_xor_reduce(void* dst, void* const* srcs, int n, uint64_t bytes, int clear_srcs, void* stream);
 
 /* ---- drain: device staging -> pinned host on a side stream ------------------------------------
  * Replaces the device-wide torch.cuda.synchronize() stall of async_ckpt/torch_ckpt.py:50,

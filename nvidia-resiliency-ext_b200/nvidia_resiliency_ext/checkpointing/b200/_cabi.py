@@ -12,7 +12,7 @@ import os
 from pathlib import Path
 from typing import Optional
 
-ABI_VERSION = 6
+ABI_VERSION = 7
 
 OK = 0
 E_INVALID = 1000
@@ -56,6 +56,7 @@ EXPORTED_SYMBOLS = (
     "nvrx_pack_sharded",
     "nvrx_plan_set_shard_rotation",
     "nvrx_pack_broadcast",
+    "nvrx_xor_reduce",
     "nvrx_drain",
     "nvrx_snapshot",
     "nvrx_snapshot_range",
@@ -169,6 +170,7 @@ def _declare(lib: C.CDLL) -> None:
         "nvrx_pack_sharded": (_int, [_vp, _vp, P(_vp), _int, _u64, _u64, _vp]),
         "nvrx_plan_set_shard_rotation": (_int, [_vp, _u32]),
         "nvrx_pack_broadcast": (_int, [_vp, P(_vp), _int, _u64, _vp]),
+        "nvrx_xor_reduce": (_int, [_vp, P(_vp), _int, _u64, _int, _vp]),
         "nvrx_drain": (_int, [_vp, _vp, _u64, _u64, _vp, _u64, _vp, _vp]),
         "nvrx_snapshot": (_int, [_vp, _vp, _vp, _u64, _vp, _u64, _vp, _vp, _vp, _vp]),
         "nvrx_snapshot_range": (_int, [_vp, _i64, _i64, _vp, _vp, _u64, _vp, _u64, _vp, _vp, _vp, _vp]),

@@ -102,6 +102,7 @@ def shared_exchange(engine: SnapshotEngine, group, need: int):
             if have is not None:
                 have.close()
             have = engine._exchange_buf = DeviceBuffer(max(target, 512), engine.device)
+            engine._exchange_dirty = False  # zero-filled (parity saves rely on it)
         p2p_ok = mode != "nccl" and group.world_size > 1
         p2p_ok = p2p_ok and all(i["host"] == infos[me]["host"] and i["boot"] == infos[me]["boot"] for i in infos)
         p2p_ok = p2p_ok and all(r == me or torch.cuda.can_device_access_peer(engine.device, i["dev"]) for r, i in enumerate(infos))
@@ -130,6 +131,14 @@ def _boot_id() -> str:
             return f.read().strip()
     except OSError:
         return ""
+
+
+def xor_reduce(engine: SnapshotEngine, dst: int, srcs: Sequence[int], nbytes: int, clear: bool, stream: int) -> None:
+    """``dst[0, nbytes) = XOR of the ranges at srcs`` with ONE kernel launch on ``stream`` (``nvrx_xor_reduce``); ``clear``
+    zeroes the sources in the same pass."""
+    arr = (C.c_void_p * len(srcs))(*srcs)
+    check(engine.lib.nvrx_xor_reduce(dst, arr, len(srcs), nbytes, int(clear), stream), "nvrx_xor_reduce")
+    engine.launches += 1 if nbytes else 0
 
 
 def _clique_barrier(engine: SnapshotEngine, group) -> None:
@@ -357,6 +366,7 @@ def allgather_packed(group, my_tensors: Sequence[torch.Tensor], all_placeholders
 
         stream_wait_event(stream, free_ev)  # previous drain of the exchange buffer must be over
     whole = as_uint8_tensor(xbuf.ptr, world * slot_bytes, engine.device)
+    engine._exchange_dirty = True
     if bases is not None:
         # fused pack + all-gather: ONE kernel reads the tensors once and stores slice `me` into every member's
         # exchange buffer (own HBM + NVLink P2P).  Barrier 1: every member's previous drain of its buffer is over;

@@ -311,6 +311,7 @@ class ShardedLocalCheckpointManager(LocalCheckpointManager):
         stream = engine._current_stream()
         staging = engine._ensure_staging(total)
         xbuf, bases = xch.shared_exchange(engine, self.clique, n * frag_slot)
+        engine._exchange_dirty = True
         if engine._staging_free is not None:
             stream_wait_event(stream, engine._staging_free)
         free_ev = getattr(engine, "_exchange_free", None)
@@ -436,9 +437,16 @@ class ShardedLocalCheckpointManager(LocalCheckpointManager):
             lo, hi = fragment_range(total, sb, k)
             if hi > lo:
                 dist.recv(whole[lo:hi], self._fragment_holder(owner, k), group=self.clique.group)
+        return self._scatter_image(skeleton, layout, total, whole, staging if on_gpu else None)
+
+    def _scatter_image(self, skeleton: TensorAwareStateDict, layout: dict, total: int, whole: torch.Tensor, staging):
+        """Owner side of a rebuild: its packed image (``whole`` on the host, or device ``staging``) into its skeleton."""
         skeleton.init_tensors()
         dests = list(skeleton.tensors)
-        if on_gpu:
+        if staging is not None:
+            from ...b200.engine import SnapshotEngine
+
+            engine = SnapshotEngine.get()
             here = torch.device("cuda", torch.cuda.current_device())
             fixed = [torch.empty_like(d, device=here) if (not d.is_cuda or d.device != here) else d for d in dests]
             if any(f is not d for f, d in zip(fixed, dests)):
