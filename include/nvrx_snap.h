@@ -34,7 +34,7 @@
 extern "C" {
 #endif
 
-#define NVRX_ABI_VERSION 7
+#define NVRX_ABI_VERSION 8
 
 enum {
     NVRX_OK = 0,
@@ -144,6 +144,16 @@ int nvrx_pack_broadcast(nvrx_plan* plan, void* const* peer_bases, int n_peers, u
  * 1 <= n <= 64, dst must not overlap any source; otherwise NVRX_E_INVALID.  bytes may exceed 2^32; bytes == 0 launches
  * nothing.  Algorithmic HBM bytes: (n + 1) * bytes, (2n + 1) * bytes with clearing. */
 int nvrx_xor_reduce(void* dst, void* const* srcs, int n, uint64_t bytes, int clear_srcs, void* stream);
+/* dsts[d][0, bytes) = XOR over s of coef[d*n_src + s] * srcs[s][0, bytes) in GF(2^8) with the polynomial
+ * x^8+x^4+x^3+x^2+1 (0x11d): the Reed-Solomon parity of a clique that keeps m >= 2 parity fragments, and its decode.
+ * 1 <= n_dst <= 4, 1 <= n_src <= 64; device pointers 16-byte aligned, bytes % 16 == 0, no destination overlaps a source
+ * or another destination; otherwise NVRX_E_INVALID and nothing is launched.  clear_srcs != 0: every source range is
+ * zero afterwards.  Every source is read once per launch whatever the number of destinations; a coefficient 0 skips the
+ * source for that row, 1 is a plain XOR.  One launch on `stream` (on the current device); bytes may exceed 2^32;
+ * bytes == 0 launches nothing.  Algorithmic HBM bytes: (n_src + n_dst) * bytes, (2 n_src + n_dst) * bytes with
+ * clearing. */
+int nvrx_gf_combine(void* const* dsts, int n_dst, void* const* srcs, int n_src, const uint8_t* coef, uint64_t bytes,
+                    int clear_srcs, void* stream);
 
 /* ---- drain: device staging -> pinned host on a side stream ------------------------------------
  * Replaces the device-wide torch.cuda.synchronize() stall of async_ckpt/torch_ckpt.py:50,

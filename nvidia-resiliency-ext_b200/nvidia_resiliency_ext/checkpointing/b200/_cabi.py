@@ -12,7 +12,7 @@ import os
 from pathlib import Path
 from typing import Optional
 
-ABI_VERSION = 7
+ABI_VERSION = 8
 
 OK = 0
 E_INVALID = 1000
@@ -57,6 +57,7 @@ EXPORTED_SYMBOLS = (
     "nvrx_plan_set_shard_rotation",
     "nvrx_pack_broadcast",
     "nvrx_xor_reduce",
+    "nvrx_gf_combine",
     "nvrx_drain",
     "nvrx_snapshot",
     "nvrx_snapshot_range",
@@ -171,6 +172,7 @@ def _declare(lib: C.CDLL) -> None:
         "nvrx_plan_set_shard_rotation": (_int, [_vp, _u32]),
         "nvrx_pack_broadcast": (_int, [_vp, P(_vp), _int, _u64, _vp]),
         "nvrx_xor_reduce": (_int, [_vp, P(_vp), _int, _u64, _int, _vp]),
+        "nvrx_gf_combine": (_int, [P(_vp), _int, P(_vp), _int, P(C.c_uint8), _u64, _int, _vp]),
         "nvrx_drain": (_int, [_vp, _vp, _u64, _u64, _vp, _u64, _vp, _vp]),
         "nvrx_snapshot": (_int, [_vp, _vp, _vp, _u64, _vp, _u64, _vp, _vp, _vp, _vp]),
         "nvrx_snapshot_range": (_int, [_vp, _i64, _i64, _vp, _vp, _u64, _vp, _u64, _vp, _vp, _vp, _vp]),

@@ -141,6 +141,19 @@ def xor_reduce(engine: SnapshotEngine, dst: int, srcs: Sequence[int], nbytes: in
     engine.launches += 1 if nbytes else 0
 
 
+def gf_combine(engine: SnapshotEngine, dsts: Sequence[int], srcs: Sequence[int], coef, nbytes: int, clear: bool, stream: int) -> None:
+    """``dsts[d][0, nbytes) = sum over s of coef[d][s] * srcs[s]`` in GF(2^8) with ONE kernel launch on ``stream``
+    (``nvrx_gf_combine``); ``coef`` is a ``len(dsts) x len(srcs)`` matrix of bytes, ``clear`` zeroes the sources in the
+    same pass."""
+    flat = bytes(int(c) for row in coef for c in row)
+    assert len(flat) == len(dsts) * len(srcs)
+    darr = (C.c_void_p * len(dsts))(*dsts)
+    sarr = (C.c_void_p * len(srcs))(*srcs)
+    carr = (C.c_uint8 * len(flat)).from_buffer_copy(flat)
+    check(engine.lib.nvrx_gf_combine(darr, len(dsts), sarr, len(srcs), carr, nbytes, int(clear), stream), "nvrx_gf_combine")
+    engine.launches += 1 if nbytes else 0
+
+
 def _clique_barrier(engine: SnapshotEngine, group) -> None:
     """Stream-ordered barrier over the clique (a 4-byte NCCL all-reduce): no CPU wait."""
     tok = getattr(engine, "_barrier_token", None)
