@@ -75,7 +75,13 @@ int nvrx_dev_alloc(int device, uint64_t bytes, void** out) {
     if (!guard.ok) return static_cast<int>(cudaErrorInvalidDevice);
     void* p = nullptr;
     NVRX_CUDA(cudaMalloc(&p, bytes ? bytes : 512));
-    cudaError_t e = cudaMemset(p, 0, bytes ? bytes : 512);
+    // The fill is over on return.  cudaMemset would only queue it on the legacy default stream, which the engine's
+    // non-blocking streams do not wait for: a reduce into a parity buffer allocated mid-save raced with its zero-fill.
+    cudaStream_t st = nullptr;
+    cudaError_t e = cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking);
+    if (e == cudaSuccess) e = cudaMemsetAsync(p, 0, bytes ? bytes : 512, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (st) cudaStreamDestroy(st);
     if (e != cudaSuccess) {
         cudaFree(p);
         return static_cast<int>(e);

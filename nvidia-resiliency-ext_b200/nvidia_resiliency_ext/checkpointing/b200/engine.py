@@ -182,7 +182,8 @@ class Plan:
 
 
 class DeviceBuffer:
-    """cudaMalloc'ed, zero-filled, IPC-exportable device memory (``nvrx_dev_alloc``)."""
+    """cudaMalloc'ed, IPC-exportable device memory (``nvrx_dev_alloc``), zero-filled before the constructor returns: work
+    queued afterwards on any stream sees zeros."""
 
     def __init__(self, nbytes: int, device: int):
         self._lib = _cabi.lib()

@@ -105,7 +105,10 @@ def shared_exchange(engine: SnapshotEngine, group, need: int):
             engine._exchange_dirty = False  # zero-filled (parity saves rely on it)
         p2p_ok = mode != "nccl" and group.world_size > 1
         p2p_ok = p2p_ok and all(i["host"] == infos[me]["host"] and i["boot"] == infos[me]["boot"] for i in infos)
-        p2p_ok = p2p_ok and all(r == me or torch.cuda.can_device_access_peer(engine.device, i["dev"]) for r, i in enumerate(infos))
+        # cudaDeviceCanAccessPeer never reports a device as its own peer, but ranks sharing a GPU import each other's
+        # buffers through CUDA IPC all the same
+        p2p_ok = p2p_ok and all(r == me or i["dev"] == engine.device or torch.cuda.can_device_access_peer(engine.device, i["dev"])
+                                for r, i in enumerate(infos))
         votes = group.all_gather_object((bool(p2p_ok), have.ipc_handle() if p2p_ok else None))
         if all(v[0] for v in votes):
             bases, imported = [], []

@@ -407,7 +407,7 @@ class ParityLocalCheckpointManager(ShardedLocalCheckpointManager):
                 else:
                     out = torch.from_numpy(np.concatenate(erasure.combine(step.matrix, [x.numpy() for x in srcs])))
                 for d, (owner, _) in enumerate(step.lost):
-                    dist.send(out[d * sb : (d + 1) * sb], owner, group=self.clique.group)
+                    self.clique.send_tensor(out[d * sb : (d + 1) * sb], owner)
             return None
         meta = self.clique.recv_object(survivors[0])
         sb, total, layout = meta["shard_bytes"], meta["total_bytes"], meta["layout"]
@@ -421,7 +421,7 @@ class ParityLocalCheckpointManager(ShardedLocalCheckpointManager):
             whole = torch.zeros(k * sb, dtype=torch.uint8)
         collector = {(owner, q): step.collector for step in steps for owner, q in step.lost}
         for q in range(k):
-            dist.recv(whole[q * sb : (q + 1) * sb], collector[(me, q)], group=self.clique.group)
+            self.clique.recv_tensor(whole[q * sb : (q + 1) * sb], collector[(me, q)])
         return self._scatter_image(pickle.loads(meta["skeleton"]), layout, total, whole, staging)
 
 

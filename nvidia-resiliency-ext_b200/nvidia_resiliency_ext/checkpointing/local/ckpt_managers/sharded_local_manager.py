@@ -415,9 +415,8 @@ class ShardedLocalCheckpointManager(LocalCheckpointManager):
             spec = torch.load(self._fragment_path((iteration, owner, k, n)), weights_only=False)
             if k == 0:
                 self.clique.send_object({key: spec[key] for key in ("skeleton", "layout", "total_bytes", "shard_bytes")}, owner)
-            data = spec["data"]
-            if data.numel():
-                dist.send(data.cuda() if on_gpu else data, owner, group=self.clique.group)
+            if spec["data"].numel():
+                self.clique.send_tensor(spec["data"], owner)
             return None
         meta = self.clique.recv_object(self._fragment_holder(owner, 0))
         total, sb, layout = meta["total_bytes"], meta["shard_bytes"], meta["layout"]
@@ -436,7 +435,7 @@ class ShardedLocalCheckpointManager(LocalCheckpointManager):
         for k in range(n):
             lo, hi = fragment_range(total, sb, k)
             if hi > lo:
-                dist.recv(whole[lo:hi], self._fragment_holder(owner, k), group=self.clique.group)
+                self.clique.recv_tensor(whole[lo:hi], self._fragment_holder(owner, k))
         return self._scatter_image(skeleton, layout, total, whole, staging if on_gpu else None)
 
     def _scatter_image(self, skeleton: TensorAwareStateDict, layout: dict, total: int, whole: torch.Tensor, staging):

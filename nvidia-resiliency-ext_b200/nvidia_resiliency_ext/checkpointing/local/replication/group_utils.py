@@ -342,6 +342,30 @@ class GroupWrapper:
         """Point-to-point payloads travel through GPU memory unless the backend is CPU-only."""
         return torch.device("cuda") in [torch.device(d.type) for d in self.supported_devices] and torch.cuda.is_available()
 
+    def _p2p_device(self) -> torch.device:
+        """Where ``dist.send`` / ``dist.recv`` take their tensors: gloo reduces and gathers CUDA tensors but sends and
+        receives host memory only."""
+        if self._payload_on_gpu() and self.backend != dist.Backend.GLOO:
+            return torch.device("cuda", torch.cuda.current_device())
+        return torch.device("cpu")
+
+    def send_tensor(self, tensor: torch.Tensor, dst: int) -> None:
+        """``dist.send`` of ``tensor`` to global rank ``dst``, copied to the device the backend sends from if it is not
+        there (the matching receive is :meth:`recv_tensor`)."""
+        dev = self._p2p_device()
+        dist.send(tensor if tensor.device.type == dev.type else tensor.to(dev), dst, group=self.group)
+
+    def recv_tensor(self, tensor: torch.Tensor, src: int) -> None:
+        """``dist.recv`` from global rank ``src`` into ``tensor`` (CUDA or host; contiguous), through a buffer on the
+        device the backend receives on if ``tensor`` is elsewhere."""
+        dev = self._p2p_device()
+        if tensor.device.type == dev.type:
+            dist.recv(tensor, src, group=self.group)
+            return
+        bounce = torch.empty(tensor.shape, dtype=tensor.dtype, device=dev)
+        dist.recv(bounce, src, group=self.group)
+        tensor.copy_(bounce)
+
     def execute_plan(
         self, exchange_plan: ExchangePlan, my_data: Dict[str, TensorAwareStateDict]
     ) -> Tuple[Dict[str, TensorAwareStateDict], Dict[str, float]]:

@@ -2,6 +2,7 @@
 shard + scatter restore.  Needs >= 2 GPUs (``gpurun --gpus 2``); world sizes follow the GPUs present (max 8)."""
 import hashlib
 
+import numpy as np
 import pytest
 import torch
 import torch.distributed as dist
@@ -39,6 +40,52 @@ def flat_tensors(sd):
 
     walk(sd)
     return out
+
+
+def edge_state(seed, shrink=False, device="cuda"):
+    """``rank_state`` plus a short odd-length bf16 vector and an empty tensor; ``shrink``: a smaller image than the same
+    seed's full state (one tensor gone, another shorter), so that bytes of a larger earlier save lie past its end."""
+    sd = rank_state(seed, device)
+    g = torch.Generator(device=device).manual_seed(900 + seed)
+    sd["edge"] = {"odd": torch.randn(7 + 2 * (seed % 5), device=device, generator=g).to(torch.bfloat16),
+                  "empty": torch.empty(0, 3, device=device)}
+    if shrink:
+        del sd["ids"]
+        sd["model"]["w"] = sd["model"]["w"][: 40 + seed % 13].clone()
+    return sd
+
+
+def _image(tensors, length):
+    from nvidia_resiliency_ext.checkpointing.b200.engine import expected_layout
+
+    nbytes = [t.numel() * t.element_size() for t in tensors]
+    offs, _, total = expected_layout(nbytes, [False] * len(nbytes), 512)
+    img = np.zeros(max(length, total), dtype=np.uint8)
+    for t, off, nb in zip(tensors, offs, nbytes):
+        if nb:
+            img[off : off + nb] = t.detach().cpu().contiguous().view(-1).view(torch.uint8).numpy()
+    return img, total
+
+
+def _covered(tensors):
+    """Which bytes of the packed image of ``tensors`` belong to a tensor (not to a gap or the padding)."""
+    from nvidia_resiliency_ext.checkpointing.b200.engine import expected_layout
+
+    nbytes = [t.numel() * t.element_size() for t in tensors]
+    offs, _, total = expected_layout(nbytes, [False] * len(nbytes), 512)
+    mask = np.zeros(total, dtype=bool)
+    for off, nb in zip(offs, nbytes):
+        mask[off : off + nb] = True
+    return mask
+
+
+def fill_staging(engine, value):
+    """Stale bytes all over the engine's staging (grown first, so that a later save or rebuild does not get a fresh one)."""
+    from nvidia_resiliency_ext.checkpointing.b200 import exchange as xch
+
+    st = engine._ensure_staging(16 << 20)
+    xch.as_uint8_tensor(st.ptr, st.nbytes, engine.device).fill_(value)
+    torch.cuda.synchronize()
 
 
 def _w_allgather_batch(rank, world, mode):
@@ -165,7 +212,10 @@ def test_replicated_save_retrieve_restore_full_clique(built_library, shm_dir):
     run_ranks(_w_replicated_save_and_restore, world, str(shm_dir), 1, world, tuple(range(1, world)), backend="nccl", timeout=600)
 
 
-def _w_sharded(rank, world, root, mode, kill):
+def _w_sharded(rank, world, root, mode, jump, factor, positions):
+    """Saves of ShardedLocalCheckpointManager on the device path, own file and every held fragment checked byte for byte,
+    then each lost set in ``positions`` (indices into the clique, the same in every clique) rebuilt from the fragments,
+    with a new save between them."""
     import os
     import time
 
@@ -173,35 +223,68 @@ def _w_sharded(rank, world, root, mode, kill):
     from nvidia_resiliency_ext.checkpointing.async_ckpt.core import AsyncCallsQueue
     from nvidia_resiliency_ext.checkpointing.b200.engine import SnapshotEngine
     from nvidia_resiliency_ext.checkpointing.local.basic_state_dict import BasicTensorAwareStateDict
-    from nvidia_resiliency_ext.checkpointing.local.ckpt_managers.sharded_local_manager import ShardedLocalCheckpointManager
+    from nvidia_resiliency_ext.checkpointing.local.ckpt_managers.sharded_local_manager import ShardedLocalCheckpointManager, fragment_range
 
-    mgr = ShardedLocalCheckpointManager.from_replication_params(root, replication_jump=1, replication_factor=world)
-    n = world - 1
+    mgr = ShardedLocalCheckpointManager.from_replication_params(root, replication_jump=jump, replication_factor=factor)
+    members = mgr._members
+    n = len(members) - 1
+    branch = "nccl-alltoall" if mode == "nccl" else "p2p-fused-sharded"
     q = AsyncCallsQueue(persistent=False)
-    for it in (1, 2):
-        sd = BasicTensorAwareStateDict(rank_state(rank + 10 * it))
+    engine = SnapshotEngine.get()
+
+    def save(man, it):
+        sd = BasicTensorAwareStateDict(edge_state(10 * it + rank))
         live = list(sd.tensors)
-        req = mgr.save(sd, it, is_async=True)
+        launches0 = engine.launches
+        req = man.save(sd, it, is_async=True)
+        assert engine.last_exchange == branch and engine.launches == launches0 + 1, (engine.last_exchange, engine.launches - launches0)
         q.schedule_async_request(req)
         for t in live:
-            t.zero_()
-        assert q.maybe_finalize_async_calls(blocking=True, no_dist=False) == [it - 1]
-    assert SnapshotEngine.get().last_exchange == ("nccl-alltoall" if mode == "nccl" else "p2p-fused-sharded")
+            t.zero_()  # training goes on: the files must hold the state from before
+        assert len(q.maybe_finalize_async_calls(blocking=True, no_dist=False)) == 1
+
+    def want(r, it):
+        return flat_tensors(edge_state(10 * it + r))
+
+    for it in (1, 2):
+        save(mgr, it)
     time.sleep(0.5)
     files = sorted(p.name for p in mgr.local_ckpt_dir.iterdir())
-    want = [f"iter_0000002_{rank}_local.pt"] + [f"iter_0000002_{m}_local.s{mgr._others(m).index(rank)}of{n}.pt" for m in range(world) if m != rank]
-    assert files == sorted(want), (files, want)
+    expect = [f"iter_0000002_{rank}_local.pt"] + [f"iter_0000002_{m}_local.s{mgr._others(m).index(rank)}of{n}.pt" for m in members if m != rank]
+    assert files == sorted(expect), (files, expect)
+    own = list(torch.load(mgr.local_ckpt_dir / f"iter_0000002_{rank}_local.pt", weights_only=False).tensors)
+    assert len(own) == len(want(rank, 2)) and all(bit_equal(a, b) for a, b in zip(own, want(rank, 2))), "own file"
+    for m in members:
+        if m == rank:
+            continue
+        k = mgr._others(m).index(rank)
+        img, total = _image(want(m, 2), 0)
+        spec = torch.load(mgr.local_ckpt_dir / f"iter_0000002_{m}_local.s{k}of{n}.pt", weights_only=False)
+        lo, hi = fragment_range(total, spec["shard_bytes"], k)
+        tensor_bytes = _covered(want(m, 2))[lo:hi]  # striped fragments need not clear the gaps: only tensor bytes count
+        assert spec["total_bytes"] == total and spec["data"].numel() == hi - lo, ("fragment size", m, k)
+        assert np.array_equal(spec["data"].numpy()[tensor_bytes], img[lo:hi][tensor_bytes]), ("fragment bytes", m, k)
     dist.barrier()
-    if rank in kill:
-        for p in mgr.local_ckpt_dir.iterdir():
-            p.unlink()
-    dist.barrier()
-    mgr2 = ShardedLocalCheckpointManager(root, clique=mgr.clique)
-    assert mgr2.find_latest() == 2
-    loaded, cid = mgr2.load()
-    want_t = flat_tensors(rank_state(rank + 20))
-    got = list(loaded.tensors)
-    assert cid == (2, rank, "") and len(got) == len(want_t) and all(a.is_cuda and bit_equal(a, b) for a, b in zip(got, want_t))
+
+    it = 2
+    for pos in positions:
+        lost = [members[i] for i in pos]
+        if rank in lost:
+            for p in mgr.local_ckpt_dir.glob(f"iter_{it:07d}_*"):
+                p.unlink()
+        dist.barrier()
+        fill_staging(engine, 0xCD)  # the rebuilt image must not keep staging's bytes
+        probe = ShardedLocalCheckpointManager(root, clique=mgr.clique)
+        assert probe.find_latest() == it
+        loaded, cid = probe.load()
+        got = list(loaded.tensors)
+        ref = want(rank, it)
+        assert cid == (it, rank, "") and len(got) == len(ref), (lost, rank)
+        assert all(a.is_cuda and bit_equal(a, b) for a, b in zip(got, ref)), ("rebuild", lost, rank)
+        dist.barrier()
+        it += 1
+        save(probe, it)
+        mgr = probe
     q.close()
 
 
@@ -210,4 +293,4 @@ def test_sharded_manager_all_to_all_and_rebuild(built_library, shm_dir, mode):
     """North-star layout: 1/(F-1) fragments exchanged with one all-to-all (fused into the pack kernel over NVLink P2P, or
     NCCL), a member that lost its storage is rebuilt from the fragments with the scatter kernel, bit-exact."""
     world = min(torch.cuda.device_count(), 8)
-    run_ranks(_w_sharded, world, str(shm_dir / mode), mode, (world - 1,), backend="nccl")
+    run_ranks(_w_sharded, world, str(shm_dir / mode), mode, 1, world, [(world - 1,)], backend="nccl")
