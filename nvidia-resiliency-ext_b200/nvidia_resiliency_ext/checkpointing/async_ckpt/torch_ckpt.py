@@ -83,6 +83,30 @@ class TorchAsyncCheckpoint(object):
         engine.reserve(plan.staging_bytes, len(cuda))
         return plan.staging_bytes
 
+    def load(self, f, map_location=None, *, into=None, strict: bool = True, verify: bool = False):
+        """Load a ``torch.save`` file (new; ``async_save``'s files or any other).
+
+        * ``map_location`` None or the CPU (and no ``into``): exactly ``torch.load(f, map_location=map_location)``.
+        * ``map_location`` a CUDA device of this process (``"cuda"``, ``"cuda:k"``, ``torch.device``): what
+          ``torch.load(f, map_location=that device)`` returns -- same dtypes, shapes, strides, storage offsets, bytes and
+          storage sharing, one CUDA storage per file record -- read by the snapshot engine (parallel ``pread`` -> pinned
+          ring -> HBM -> one scatter kernel; in place when ``f`` is a hard link to one of this process's pinned slots).
+        * ``into=state_dict`` of live CUDA tensors (``map_location`` None): the saved bytes are written into those tensors
+          where they are, matched by nested key path, any strides, fp32 / bf16 / fp16 converted on the device like
+          ``target.copy_(saved)``; other dtype pairs and targets on the CPU or another device are copied with ``copy_``.
+          ``strict=True`` raises on missing or unexpected keys before anything is read; shape mismatches always raise.
+          Returns ``(missing_keys, unexpected_keys)`` like ``load_state_dict``.
+        * ``verify=True``: every record read is checked against its CRC-32 field (on the GPU, over the bytes that reached
+          HBM); a mismatch raises ``SnapError("crc32 mismatch ...")`` naming the key, the file and the record offset.
+          In-place targets may hold the unverified bytes by then.  Records written without a CRC-32 are counted as
+          unverified with one warning.
+
+        The engine modes need a CUDA device and the engine library (``SnapError`` otherwise) and a path (or a file object
+        opened on one).  ``SnapshotEngine.last_torch_load`` describes the last such load."""
+        from ..b200.fastload import load
+
+        return load(f, map_location, into=into, strict=strict, verify=verify)
+
     def _reap(self, finalized=None):
         """Release the host slots of finalized calls."""
         if finalized is None:

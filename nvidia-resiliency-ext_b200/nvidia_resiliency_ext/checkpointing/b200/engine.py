@@ -916,6 +916,7 @@ class SnapshotEngine:
         self.box_loads = 0  # load_boxes() calls (torch.distributed.checkpoint loads on the engine)
         self.box_batches = 0  # staging batches of those loads (one box-scatter launch each)
         self.last_box_load: Optional[dict] = None  # batches / peak staging / algorithmic bytes (/ kernel ms) of the last one
+        self.last_torch_load: Optional[dict] = None  # bytes read / records / entries / fallbacks / launches / host ms (fastload.py)
         self._aux: Optional[Stream] = None  # checksum kernels (created on first use)
         self._pid = os.getpid()  # forked writers inherit this object; only the creator may tear it down
         # NVRX_B200_TRACE=1: host-side time stamps of the last snapshot() (enter / planned / launched), for the stall breakdown
@@ -1329,6 +1330,7 @@ class SnapshotEngine:
         resident: Optional[Tuple[_Slot, Sequence[int]]] = None,
         file_source: Optional[Tuple[str, Sequence[int]]] = None,
         expect_crcs: Optional[Sequence[int]] = None,
+        crc_names: Optional[Sequence[str]] = None,
     ) -> List[torch.Tensor]:
         """CPU tensors -> CUDA tensors of this device with one H2D copy and one scatter kernel.
 
@@ -1340,7 +1342,8 @@ class SnapshotEngine:
         ``pread`` from the checkpoint file instead of a memcpy from the tensors' mmap (no page-by-page faults).
         ``expect_crcs[i]``: crc32 the bytes of tensor i must have (from the file's directory; 0 = unknown).  The checksum
         kernel sums what actually ARRIVED in HBM, so a flipped bit in the file, the page cache, the pinned slot or on the way
-        over PCIe fails the restore (``SnapError``) instead of silently resuming training from corrupt weights."""
+        over PCIe fails the restore (``SnapError``) instead of silently resuming training from corrupt weights.
+        ``crc_names[i]``: what that error calls tensor i (default: its index)."""
         host_tensors = [t.detach() for t in host_tensors]
         target_dtypes = [
             (widen_to[i] if widen_to is not None and widen_to[i] is not None else t.dtype)
@@ -1420,9 +1423,10 @@ class SnapshotEngine:
                 crc.close()
                 bad = [i for i, (g, e, nb) in enumerate(zip(got, expect_crcs, plan.packed_nbytes)) if nb and e and g != e]
                 if bad:
+                    first = crc_names[bad[0]] if crc_names is not None else f"#{bad[0]}"
                     raise SnapError(
                         _cabi.E_STATE, "verifying restored tensors",
-                        f"crc32 mismatch on {len(bad)} of {len(out)} tensors (first: #{bad[0]}, got {got[bad[0]]:#010x}, "
+                        f"crc32 mismatch on {len(bad)} of {len(out)} tensors (first: {first}, got {got[bad[0]]:#010x}, "
                         f"file says {expect_crcs[bad[0]]:#010x}) -- the checkpoint is corrupt",
                     )
         finally:
