@@ -34,7 +34,7 @@
 extern "C" {
 #endif
 
-#define NVRX_ABI_VERSION 8
+#define NVRX_ABI_VERSION 9
 
 enum {
     NVRX_OK = 0,
@@ -183,6 +183,37 @@ int nvrx_snapshot_range(nvrx_plan* plan, int64_t seg_lo, int64_t seg_hi, void* s
  * groups of copy chunks (1, 4, 16, ... chunks; NVRX_B200_PACK_GROWTH), 4 for a 16 GB snapshot with 256 MiB chunks.  A
  * range starting at segment 0 sets the count, a later range adds its own. */
 int nvrx_plan_last_launches(const nvrx_plan* plan, uint32_t* launches);
+/* ---- staging-free snapshot: live tensors -> pinned slot, no device staging buffer -------------------------------------
+ * The reference's preload_tensors (utils.py:85-99) copies every tensor to the host on the training stream and then
+ * synchronises the device.  Here the copies run on a side stream behind an event of the training stream and read the live
+ * tensors; the caller must not write them until the done event (the "fence").
+ *
+ * nvrx_direct_schedule (no CUDA call) splits a layout of n segments (tensor-side nbytes, NVRX_SEG_* flags and slot
+ * offsets, ascending) into the segments one small pack kernel writes -- every narrowed segment and every non-empty segment
+ * below `small_bytes` -- and the ones the copy engines move, one cudaMemcpyAsync each, in offset order:
+ *   in_kernel[i]       1 for a kernel segment, else 0 (empty segments are neither: no byte to move)
+ *   progress_after[i]  for a copied segment, the slot offset the progress word reports (minus base_value) after its copy:
+ *                      the end of segment i when the copies since the previous report (this one included) move at least
+ *                      `chunk_bytes`; 0 = no report.  Kernel and empty segments always get 0.
+ * NVRX_E_INVALID on NULL arrays, offsets that are not ascending and disjoint, or an odd narrowed length. */
+int nvrx_direct_schedule(int64_t n, const uint64_t* nbytes, const uint32_t* flags, const uint64_t* offsets,
+                         uint64_t small_bytes, uint64_t chunk_bytes, uint8_t* in_kernel, uint64_t* progress_after);
+/* Enqueue one staging-free snapshot on `stream` (the engine's side stream), behind `start_event` (recorded on the training
+ * stream; may be NULL):
+ *   1. `kernel_plan` (may be NULL): a plan over the kernel segments alone, created with their slot offsets
+ *      (nvrx_plan_create_at), packed by the LDG walker with a grid of a few CTAs straight into the mapped device address of
+ *      `host_dst` (registered with cudaHostRegisterMapped).  One launch, none when the plan has no tiles.
+ *   2. n_copies cudaMemcpyAsync D2H, src[i] -> host_dst + dst_offsets[i], nbytes[i] bytes, offsets ascending; after copy i
+ *      a stream-ordered write sets *progress = base_value + progress_after[i] when that is not 0 (nvrx_direct_schedule).
+ *   3. *progress = base_value + total_bytes, then `done_event` (optional) is recorded.
+ * The kernel runs before every copy in stream order, so the progress word never reports a byte that has not landed.
+ * `done_event` is the end of every read of the source tensors.  NVRX_E_INVALID on a range past total_bytes, offsets
+ * that are not ascending, progress values that fall or lie past the end of their copy's group, or a kernel plan
+ * larger than total_bytes. */
+int nvrx_snapshot_direct(nvrx_plan* kernel_plan, int64_t n_copies, const void* const* src, const uint64_t* dst_offsets,
+                         const uint64_t* nbytes, const uint64_t* progress_after, void* host_dst, uint64_t total_bytes,
+                         volatile uint64_t* progress, uint64_t base_value, int device, void* start_event, void* stream,
+                         void* done_event);
 /* Mirror for restore: pinned host -> device staging (H2D), optional event. */
 int nvrx_fill(void* staging, const void* host_src, uint64_t bytes, uint64_t chunk_bytes, void* stream,
               void* done_event);

@@ -780,6 +780,94 @@ int nvrx_snapshot_range(nvrx_plan* p, int64_t seg_lo, int64_t seg_hi, void* stag
     return NVRX_OK;
 }
 
+int nvrx_direct_schedule(int64_t n, const uint64_t* nbytes, const uint32_t* flags, const uint64_t* offsets,
+                         uint64_t small_bytes, uint64_t chunk_bytes, uint8_t* in_kernel, uint64_t* progress_after) {
+    if (n < 0 || (n > 0 && (!nbytes || !offsets || !in_kernel || !progress_after))) return NVRX_E_INVALID;
+    uint64_t prev_end = 0, group = 0;
+    for (int64_t i = 0; i < n; ++i) {
+        const bool narrow = flags && (flags[i] & NVRX_SEG_NARROW_F32_BF16);
+        if (narrow && (nbytes[i] & 3u)) return NVRX_E_INVALID;
+        const uint64_t packed = narrow ? nbytes[i] / 2 : nbytes[i];
+        if (offsets[i] < prev_end) return NVRX_E_INVALID;
+        prev_end = offsets[i] + packed;
+        in_kernel[i] = packed != 0 && (narrow || nbytes[i] < small_bytes);
+        progress_after[i] = 0;
+        if (packed == 0 || in_kernel[i]) continue;
+        group += packed;
+        if (group >= chunk_bytes) {
+            progress_after[i] = prev_end;
+            group = 0;
+        }
+    }
+    return NVRX_OK;
+}
+
+int nvrx_snapshot_direct(nvrx_plan* kp, int64_t n_copies, const void* const* src, const uint64_t* dst_offsets,
+                         const uint64_t* nbytes, const uint64_t* progress_after, void* host_dst, uint64_t total_bytes,
+                         volatile uint64_t* progress, uint64_t base_value, int device, void* start_event, void* stream,
+                         void* done_event) {
+    if (n_copies < 0 || (n_copies > 0 && (!src || !dst_offsets || !nbytes || !progress_after))) return NVRX_E_INVALID;
+    if (total_bytes && !host_dst) return NVRX_E_INVALID;
+    if (kp && (kp->staging_bytes > total_bytes || kp->device != device)) return NVRX_E_INVALID;
+    uint64_t prev_end = 0, reported = 0;
+    for (int64_t i = 0; i < n_copies; ++i) {
+        const uint64_t end = dst_offsets[i] + nbytes[i];
+        if ((nbytes[i] && !src[i]) || dst_offsets[i] < prev_end || end < dst_offsets[i] || end > total_bytes)
+            return NVRX_E_INVALID;
+        // a report may only name bytes that have landed: at most the end of this copy, never below an earlier report
+        if (progress_after[i] && (progress_after[i] > end || progress_after[i] < reported)) return NVRX_E_INVALID;
+        if (progress_after[i]) reported = progress_after[i];
+        prev_end = end;
+    }
+    DeviceGuard guard(device);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (start_event) NVRX_CUDA(cudaStreamWaitEvent(st, static_cast<cudaEvent_t>(start_event), 0));
+    void* prog_dev = nullptr;
+    if (progress) NVRX_CUDA(cudaHostGetDevicePointer(&prog_dev, const_cast<uint64_t*>(progress), 0));
+    if (kp) {
+        kp->last_launches = 0;
+        if (kp->shard_bytes) {
+            kp->shard_bytes = 0;
+            int rc = build_tiles(kp);
+            if (rc) return rc;
+        }
+        if (kp->n_tiles) {
+            void* dev_dst = nullptr;
+            NVRX_CUDA(cudaHostGetDevicePointer(&dev_dst, host_dst, 0));
+            if (reinterpret_cast<uintptr_t>(dev_dst) & 511u) return NVRX_E_INVALID;
+            int rc = upload(kp, st);
+            if (rc) return rc;
+            // Always the LDG walker: its 16-byte stores are ordinary st.global, which reach mapped host memory like device
+            // memory; the TMA ring's bulk stores to system memory were never validated.  The grid stays at a few CTAs
+            // because the kernel runs beside the training kernels and its bytes are a small share of the snapshot.
+            constexpr uint32_t kDirectCtas = 8;
+            const TileSpan span = whole_span(kp);
+            const uint32_t grid = std::max<uint32_t>(1, std::min<uint32_t>(kDirectCtas, span.na + span.nb));
+            PeerMap pm;
+            memset(&pm, 0, sizeof(pm));
+            nvrx::walk_ldg<nvrx::kDirPack><<<grid, nvrx::kLdgThreads, 0, st>>>(kp->d_segs, span, static_cast<uint8_t*>(dev_dst), pm);
+            NVRX_CUDA(cudaGetLastError());
+            if (!kp->last_launch) NVRX_CUDA(cudaEventCreateWithFlags(&kp->last_launch, cudaEventDisableTiming));
+            NVRX_CUDA(cudaEventRecord(kp->last_launch, st));
+            kp->last_launches = 1;
+        }
+    }
+    uint8_t* const dst = static_cast<uint8_t*>(host_dst);
+    for (int64_t i = 0; i < n_copies; ++i) {
+        if (nbytes[i]) NVRX_CUDA(cudaMemcpyAsync(dst + dst_offsets[i], src[i], nbytes[i], cudaMemcpyDeviceToHost, st));
+        if (prog_dev && progress_after[i]) {
+            int rc = nvrx_stream_write_u64(st, prog_dev, base_value + progress_after[i]);
+            if (rc) return rc;
+        }
+    }
+    if (prog_dev) {
+        int rc = nvrx_stream_write_u64(st, prog_dev, base_value + total_bytes);
+        if (rc) return rc;
+    }
+    if (done_event) NVRX_CUDA(cudaEventRecord(static_cast<cudaEvent_t>(done_event), st));
+    return NVRX_OK;
+}
+
 int nvrx_plan_last_launches(const nvrx_plan* p, uint32_t* launches) {
     if (!p || !launches) return NVRX_E_INVALID;
     *launches = p->last_launches;

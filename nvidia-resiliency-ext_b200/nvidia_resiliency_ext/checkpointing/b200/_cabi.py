@@ -12,7 +12,7 @@ import os
 from pathlib import Path
 from typing import Optional
 
-ABI_VERSION = 8
+ABI_VERSION = 9
 
 OK = 0
 E_INVALID = 1000
@@ -62,6 +62,8 @@ EXPORTED_SYMBOLS = (
     "nvrx_snapshot",
     "nvrx_snapshot_range",
     "nvrx_plan_last_launches",
+    "nvrx_direct_schedule",
+    "nvrx_snapshot_direct",
     "nvrx_fill",
     "nvrx_fill_from_fd",
     "nvrx_boxplan_create",
@@ -177,6 +179,10 @@ def _declare(lib: C.CDLL) -> None:
         "nvrx_snapshot": (_int, [_vp, _vp, _vp, _u64, _vp, _u64, _vp, _vp, _vp, _vp]),
         "nvrx_snapshot_range": (_int, [_vp, _i64, _i64, _vp, _vp, _u64, _vp, _u64, _vp, _vp, _vp, _vp]),
         "nvrx_plan_last_launches": (_int, [_vp, P(_u32)]),
+        "nvrx_direct_schedule": (_int, [_i64, P(_u64), P(_u32), P(_u64), _u64, _u64, P(C.c_uint8), P(_u64)]),
+        "nvrx_snapshot_direct": (
+            _int, [_vp, _i64, P(_vp), P(_u64), P(_u64), P(_u64), _vp, _u64, _vp, _u64, _int, _vp, _vp, _vp]
+        ),
         "nvrx_fill": (_int, [_vp, _vp, _u64, _u64, _vp, _vp]),
         "nvrx_fill_from_fd": (_int, [_vp, _u64, _int, _i64, P(_u64), P(_u64), P(_u64), _u64, _int, _int, _int, _vp]),
         "nvrx_boxplan_create": (

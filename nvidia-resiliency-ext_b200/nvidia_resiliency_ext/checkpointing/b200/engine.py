@@ -40,6 +40,13 @@ logger = logging.getLogger(__name__)
 
 DEFAULT_ALIGN = 512
 DEFAULT_DRAIN_CHUNK = int(os.environ.get("NVRX_B200_DRAIN_CHUNK_MB", "256")) << 20
+# Staging-free snapshots: segments below this size are written by one small pack kernel (8 CTAs, straight into the mapped
+# slot) instead of a copy-engine D2H each.  bench_direct_snapshot.py's sweep on an H100 80GB HBM3 (700 W), 256 tensors of one
+# size, from the call to the end of the side stream: 4 B 1162 us by copies / 483 us by the kernel, 64 KiB 1434 / 522 us,
+# 256 KiB 2386 / 1983 us, 1 MiB 6307 / 5542 us.  Every copy costs a few microseconds of its own, and the kernel stayed
+# ahead up to the largest size measured, so the bound sits there.  On the C2 state it sends the 291 step scalars and the 260
+# norm weights to the kernel and every other tensor (2 MiB and up) to the copy engines.
+DIRECT_SMALL_BYTES = 1 << 20
 
 
 def _ptr_array(values: Sequence[int]):
@@ -733,6 +740,11 @@ class Snapshot:
     pack_stop: Optional[Event] = None
     released: bool = False
     crc_info: Optional[dict] = None  # where the GPU's checksum values land in the slot (opt-in, see gpu_crc_enabled)
+    # staging-free snapshots (``snapshot(direct=True)``): the tensors the copies read, held until release() so that the
+    # caching allocator cannot hand their blocks to other work while the copies still read them, and the event that ends
+    # those reads (the slot's done event)
+    sources: List[torch.Tensor] = field(default_factory=list)
+    read_done: Optional[Event] = None
 
     def drained(self) -> bool:
         return self.slot.done_event.query()
@@ -772,6 +784,7 @@ class Snapshot:
     def release(self) -> None:
         if not self.released:
             self.released = True
+            self.sources = []
             self.engine._release(self.slot)
 
 
@@ -918,6 +931,7 @@ class SnapshotEngine:
         self.last_box_load: Optional[dict] = None  # batches / peak staging / algorithmic bytes (/ kernel ms) of the last one
         self.last_torch_load: Optional[dict] = None  # bytes read / records / entries / fallbacks / launches / host ms (fastload.py)
         self._aux: Optional[Stream] = None  # checksum kernels (created on first use)
+        self._direct_start: Optional[Event] = None  # start of a staging-free snapshot on the current stream (reused)
         self._pid = os.getpid()  # forked writers inherit this object; only the creator may tear it down
         # NVRX_B200_TRACE=1: host-side time stamps of the last snapshot() (enter / planned / launched), for the stall breakdown
         self.trace: Optional[dict] = {} if os.environ.get("NVRX_B200_TRACE", "0") == "1" else None
@@ -1003,15 +1017,17 @@ class SnapshotEngine:
         """Slots a snapshot could go to without giving up a published checkpoint: idle unpublished ones plus pool headroom."""
         return spare_slots(self._slots, self.max_host_slots)
 
-    def reserve(self, nbytes: int, n_tensors: int = 0) -> None:
+    def reserve(self, nbytes: int, n_tensors: int = 0, *, staging: bool = True) -> None:
         """Pre-allocate staging and every host slot for snapshots of up to ``nbytes`` packed bytes of ``n_tensors``
         tensors (pinning 16 GB takes seconds; do it once at start-up instead of inside the first save).  With zero-copy
         persistence on, a slot also holds the checkpoint file's small records and directory behind the payload: that
-        room is reserved too, or the first save would re-create and re-pin the slot."""
+        room is reserved too, or the first save would re-create and re-pin the slot.  ``staging=False``: the slots only
+        (staging-free snapshots, ``snapshot(direct=True)``, never use staging)."""
         from .fastsave import zero_copy_enabled
         from .ptzip import slot_tail_room
 
-        self._ensure_staging(nbytes)
+        if staging:
+            self._ensure_staging(nbytes)
         slot_bytes = nbytes + (slot_tail_room(n_tensors) if zero_copy_enabled() else 0)
         for s in self._slots:
             if not s.busy and not s.published():
@@ -1076,13 +1092,18 @@ class SnapshotEngine:
         return plan, container
 
     # ---- snapshot -------------------------------------------------------------------------------
-    def snapshot(self, tensors: Iterable[torch.Tensor], *, narrow: bool = False, container: Optional[bool] = None) -> Snapshot:
+    def snapshot(self, tensors: Iterable[torch.Tensor], *, narrow: bool = False, container: Optional[bool] = None,
+                 direct: bool = False) -> Snapshot:
         """Pack ``tensors`` (CUDA tensors of this device; others pass through) and start the drain.
 
         Returns as soon as the pack kernel and the side-stream copy are *enqueued*.  ``container`` (default: the
         ``NVRX_B200_ZERO_COPY`` switch) packs in checkpoint-container geometry, see :meth:`_plan_for`.  ``tensors`` may be
         a lazy walk: when it has the structure of the previous snapshot, the first staging range is launched as soon as its
-        tensors are checked, and the later ranges are checked while it packs (:meth:`_snapshot_staged`)."""
+        tensors are checked, and the later ranges are checked while it packs (:meth:`_snapshot_staged`).
+
+        ``direct=True``: a staging-free snapshot (:meth:`_snapshot_direct`).  The bytes go from the live tensors to the slot
+        on the side stream, so NO kernel may write a saved tensor until ``Snapshot.read_done`` has completed on the device
+        (reads are fine)."""
         trace = self.trace
         if trace is not None:
             trace.clear()
@@ -1091,6 +1112,8 @@ class SnapshotEngine:
             from .fastsave import zero_copy_enabled
 
             container = zero_copy_enabled()
+        if direct:
+            return self._snapshot_direct(tensors if isinstance(tensors, list) else list(tensors), narrow, container)
         staged = self._staged_plan(narrow, container)
         if staged is not None:
             return self._snapshot_staged(staged[0], staged[1], iter(tensors), narrow, container)
@@ -1274,6 +1297,100 @@ class SnapshotEngine:
         self._staging_free = slot.done_event
         return self._finish_snapshot(plan, slot, staging, crc, crc_off, ready_off, packed_ev, cuda_tensors, mask, passthrough,
                                      len(all_tensors), start, stop)
+
+    def _direct_schedule(self, plan: Plan) -> dict:
+        """How a staging-free snapshot of ``plan``'s layout moves its segments (``nvrx_direct_schedule``), cached on the plan:
+        the plan of the kernel segments at their slot offsets (None when there are none), the copied segments and their
+        slot offsets, sizes and progress reports."""
+        cached = plan.__dict__.get("_direct")
+        if cached is not None and cached["key"] == (self.drain_chunk, DIRECT_SMALL_BYTES):
+            return cached
+        n = plan.n
+        flags = plan.__dict__["_flags"]
+        in_kernel, after = (C.c_uint8 * max(n, 1))(), (C.c_uint64 * max(n, 1))()
+        check(
+            self.lib.nvrx_direct_schedule(
+                n, _u64_array(plan.nbytes), _u32_array(flags), _u64_array(plan.offsets), DIRECT_SMALL_BYTES,
+                self.drain_chunk, in_kernel, after,
+            ),
+            "nvrx_direct_schedule",
+        )
+        small = [i for i in range(n) if in_kernel[i]]
+        copies = [i for i in range(n) if not in_kernel[i] and plan.packed_nbytes[i]]
+        kernel = None
+        if small:
+            kernel = Plan(
+                [plan.ptrs[i] for i in small], [plan.nbytes[i] for i in small], [flags[i] for i in small], device=self.device,
+                align=self.align, tile_bytes=self.tile_bytes, variant=_cabi.VARIANT_LDG,
+                staging_offsets=[plan.offsets[i] for i in small],
+            )
+        cached = plan.__dict__["_direct"] = {
+            "key": (self.drain_chunk, DIRECT_SMALL_BYTES), "kernel": kernel, "small": small, "copies": copies,
+            "dst": _u64_array([plan.offsets[i] for i in copies]), "nbytes": _u64_array([plan.nbytes[i] for i in copies]),
+            "after": _u64_array([after[i] for i in copies]),
+        }
+        return cached
+
+    def _snapshot_direct(self, all_tensors: List[torch.Tensor], narrow: bool, container: bool) -> Snapshot:
+        """Staging-free snapshot: one native call (``nvrx_snapshot_direct``) enqueues, on the side stream behind an event of
+        the current stream, one small LDG pack of the narrowed and small segments straight into the mapped slot, then one
+        copy-engine D2H per other segment from the live tensor into the slot, in slot-offset order, with the progress word
+        advanced every ``drain_chunk`` bytes.  The slot layout is the one :meth:`_snapshot_all` would use, so writers,
+        ``descriptor()``, publishing and slot reuse are the same; staging is never allocated.  The current stream carries
+        one event record.  Passthrough host tensors, the device check and the compaction of non-contiguous tensors are
+        those of :meth:`_snapshot_all`; the compacted temporaries are among the sources the snapshot holds."""
+        if gpu_crc_enabled():
+            raise ValueError("NVRX_B200_GPU_CRC=1 checksums the staging buffer, which a staging-free snapshot does not have")
+        dev = self.device
+        passthrough: Dict[int, torch.Tensor] = {}
+        cuda_tensors = all_tensors
+        if not all([t.get_device() == dev for t in all_tensors]):
+            passthrough = {i: t for i, t in enumerate(all_tensors) if t.get_device() != dev}
+            if any(t.is_cuda for t in passthrough.values()):
+                raise ValueError("snapshot: the CUDA tensors must live on one device (the engine's)")
+            cuda_tensors = [t for i, t in enumerate(all_tensors) if i not in passthrough]
+        if not all([t.is_contiguous() for t in cuda_tensors]):
+            cuda_tensors = [t if t.is_contiguous() else t.detach().contiguous() for t in cuda_tensors]
+        mask = self._narrow_mask(cuda_tensors, narrow) if narrow else None
+        container = bool(container) and not passthrough and len(cuda_tensors) > 0 and self._spare_slots() > 1
+        plan = self._plan_for(cuda_tensors, mask, container)
+        if "_flags" not in plan.__dict__:
+            plan.__dict__["_flags"] = [_cabi.SEG_NARROW_F32_BF16 if mask is not None and nr else 0
+                                       for nr in (mask if mask is not None else [False] * plan.n)]
+        sched = self._direct_schedule(plan)
+        kernel = sched["kernel"]
+        if kernel is not None:
+            kernel.update_ptrs([plan.ptrs[i] for i in sched["small"]])
+        src = _ptr_array([plan.ptrs[i] for i in sched["copies"]])
+        stream = self._current_stream()
+        if self._direct_start is None:
+            self._direct_start = Event(dev)
+        self._direct_start.record(stream)  # after the compaction: everything queued so far belongs to the snapshot
+        tail_room = 0
+        if container:
+            from .ptzip import slot_tail_room
+
+            tail_room = slot_tail_room(len(cuda_tensors))
+        slot = self._acquire_slot(plan.staging_bytes + tail_room)
+        base = slot.drained_total
+        try:
+            check(
+                self.lib.nvrx_snapshot_direct(
+                    kernel._h if kernel is not None else None, len(sched["copies"]), src, sched["dst"], sched["nbytes"],
+                    sched["after"], slot.buf.data_ptr, plan.staging_bytes, slot.buf.progress_ptr, base, dev,
+                    self._direct_start.handle, self._side.handle, slot.done_event.handle,
+                ),
+                "nvrx_snapshot_direct",
+            )
+        except BaseException:
+            self._release(slot)
+            raise
+        self.launches += kernel.last_launches() if kernel is not None else 0
+        slot.drained_total = base + plan.staging_bytes
+        snap = self._finish_snapshot(plan, slot, None, None, 0, 0, None, cuda_tensors, mask, passthrough, len(all_tensors))
+        snap.sources = list(cuda_tensors)
+        snap.read_done = slot.done_event
+        return snap
 
     def _finish_snapshot(self, plan, slot, staging, crc, crc_off, ready_off, packed_ev, cuda_tensors, mask, passthrough,
                          n_total, start=None, stop=None) -> Snapshot:
