@@ -443,7 +443,9 @@ def _views_of_exchange_slot(engine: SnapshotEngine, geo: dict, slot):
 
 
 def send_packed(group, tensors: Sequence[torch.Tensor], dst_global_rank: int) -> None:
-    """Pack ``tensors`` (CUDA, or CPU which are staged through the device first) and send ONE message."""
+    """Pack ``tensors`` (CUDA, or CPU which are staged through the device first) and send ONE message.  The message
+    leaves through ``group.send_tensor``: from the device on NCCL, through host memory on gloo (which sends host memory
+    only)."""
     dev = torch.cuda.current_device()
     engine = SnapshotEngine.get(dev)
     cuda_tensors = [t if t.is_cuda else t.to(torch.device("cuda", dev)) for t in tensors]
@@ -453,19 +455,20 @@ def send_packed(group, tensors: Sequence[torch.Tensor], dst_global_rank: int) ->
     stream = engine._current_stream()
     plan.pack(xbuf.ptr, stream)
     engine.launches += 1 if plan.n_tiles else 0
-    dist.send(as_uint8_tensor(xbuf.ptr, plan.staging_bytes, dev), dst_global_rank, group=group.group)
+    group.send_tensor(as_uint8_tensor(xbuf.ptr, plan.staging_bytes, dev), dst_global_rank)
 
 
 def recv_packed(group, dests: Sequence[torch.Tensor], src_global_rank: int) -> None:
     """Receive ONE packed message and scatter it into ``dests`` (CUDA tensors, or CPU tensors filled through a
-    device bounce as the reference does at ``group_utils.py:442-446``)."""
+    device bounce as the reference does at ``group_utils.py:442-446``).  The message arrives through
+    ``group.recv_tensor``: straight into device memory on NCCL, through a host buffer on gloo."""
     dev = torch.cuda.current_device()
     engine = SnapshotEngine.get(dev)
     on_dev = [d if d.is_cuda else torch.empty(d.shape, dtype=d.dtype, device=torch.device("cuda", dev)) for d in dests]
     assert all(d.is_contiguous() for d in on_dev)
     plan = engine._plan_for(on_dev, [False] * len(on_dev))
     xbuf = _private_buffer(engine, plan.staging_bytes)
-    dist.recv(as_uint8_tensor(xbuf.ptr, plan.staging_bytes, dev), src_global_rank, group=group.group)
+    group.recv_tensor(as_uint8_tensor(xbuf.ptr, plan.staging_bytes, dev), src_global_rank)
     stream = engine._current_stream()
     plan.scatter(xbuf.ptr, stream)
     engine.launches += 1 if plan.n_tiles else 0

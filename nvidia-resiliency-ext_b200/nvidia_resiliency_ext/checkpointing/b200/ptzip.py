@@ -359,7 +359,9 @@ def publish_slot(
         file_size = os.fstat(fd).st_size
         if lay.end + tail_size(SLOT_ARCHIVE, small, len(sizes)) > file_size:
             return False
-        write_container(fd, lay, small, file_size=file_size, crcs=crcs, pad_crc=False)
+        # with checksummed storages the pad is checksummed too (up to _PAD_CRC_LIMIT, as in a copied file): a record with
+        # a zero checksum makes zipfile.testzip() / unzip -t report the whole checkpoint as corrupt
+        write_container(fd, lay, small, file_size=file_size, crcs=crcs, pad_crc=crcs is not None)
     finally:
         os.close(fd)
     # temporary link name: keeps the target's extension so that a manager's cleanup glob (iter_*_local*.pt) also removes a

@@ -3,6 +3,7 @@ device replaced at the C-ABI boundary (tests/_fake_device.py).  Covers what test
 CliqueReplicationStrategy, lose a rank's files, find_latest, retrieve, restore -- for the default one-shot exchange and for the
 modes written after the round's GPU budget was spent (streamed exchange, replicated zero-copy)."""
 import os
+import zipfile
 
 import pytest
 import torch
@@ -85,6 +86,8 @@ def _worker(rank, world, root, mode, zero_copy, kill):
                         assert a.dtype == b.dtype and torch.equal(plain(a), b), (rank, m)
                     if zero_copy:
                         assert os.stat(path).st_nlink == 2, "replica file is expected to be a hard link to a slot"
+                        with zipfile.ZipFile(path) as z:
+                            assert z.testzip() is None, f"{path.name}: a record fails its CRC-32"
                 assert len(engine._slots) <= engine.max_host_slots
             dist.barrier()
             if rank in kill:
@@ -111,6 +114,79 @@ def test_replicated_save_lose_a_rank_and_restore(shm_dir, built_library, mode, z
 
 def test_replicated_three_members_streamed(shm_dir, built_library):
     run_ranks(_worker, 3, str(shm_dir), "stream", False, (0, 2), timeout=300)
+
+
+def _p2p_routing_worker(rank, world):
+    """Rank 0 sends a state dict to rank 1 with isend_state_dict over gloo.  The packed exchange buffer looks like device
+    memory here (as it is on a GPU): every tensor that reaches ``dist.send`` / ``dist.recv`` must be a host tensor, since
+    gloo sends and receives host memory only."""
+    import ctypes as C
+
+    import torch.distributed as dist
+
+    from _fake_device import FakeCudaTensor, fake_device, plain
+    from oracle import snapshot_oracle as orc
+
+    mp = pytest.MonkeyPatch()
+    try:
+        with fake_device(mp) as (engine, lib):
+            from nvidia_resiliency_ext.checkpointing.b200 import exchange as xch
+            from nvidia_resiliency_ext.checkpointing.local.basic_state_dict import BasicTensorAwareStateDict
+            from nvidia_resiliency_ext.checkpointing.local.replication.group_utils import GroupWrapper
+
+            def device_bytes(ptr, nbytes, device):
+                return FakeCudaTensor.wrap(torch.frombuffer((C.c_uint8 * max(nbytes, 1)).from_address(ptr), dtype=torch.uint8)[:nbytes])
+
+            def to(self, *args, **kwargs):
+                dev = kwargs.get("device", args[0] if args else None)
+                if isinstance(dev, (str, torch.device)) and torch.device(dev).type == "cpu":
+                    return plain(self).clone()  # a device-to-host copy
+                return FakeCudaTensor.wrap(torch.Tensor.to(plain(self), *args, **kwargs))
+
+            class _S:
+                cuda_stream = 0
+
+                def synchronize(self):
+                    pass
+
+            seen = []
+
+            def spy(real):
+                def call(tensor, *args, **kwargs):
+                    seen.append((real.__name__, tensor.is_cuda, tensor.numel()))
+                    return real(plain(tensor), *args, **kwargs)
+
+                return call
+
+            mp.setattr(xch, "as_uint8_tensor", device_bytes)
+            mp.setattr(FakeCudaTensor, "to", to, raising=False)
+            mp.setattr(torch.cuda, "current_stream", lambda *a, **k: _S())
+            mp.setattr(dist, "send", spy(dist.send))
+            mp.setattr(dist, "recv", spy(dist.recv))
+
+            gw = GroupWrapper()
+            assert gw.backend == "gloo" and gw._payload_on_gpu()
+            want = orc.flatten_tensors(_rank_state(0, None))
+            if rank == 0:
+                gw.isend_state_dict(BasicTensorAwareStateDict(_rank_state(0, FakeCudaTensor.wrap)), 1)
+                assert lib.calls.count("pack") == 1
+            else:
+                got, log = gw.irecv_state_dict(0)
+                tensors = list(got.tensors)
+                assert lib.calls.count("scatter") == 1
+                assert log["data_recv"] == sum(t.nbytes for t in want)
+                assert len(tensors) == len(want)
+                assert all(t.is_cuda and t.dtype == w.dtype and torch.equal(plain(t), w) for t, w in zip(tensors, want))
+            payload = [s for s in seen if s[2] >= sum(t.nbytes for t in want)]
+            assert [s[0] for s in payload] == ["send" if rank == 0 else "recv"], seen
+            assert not any(is_cuda for _, is_cuda, _ in seen), f"a device tensor was handed to gloo: {seen}"
+    finally:
+        mp.undo()
+
+
+def test_gloo_point_to_point_payload_goes_through_host_memory(built_library):
+    """``send_packed`` / ``recv_packed`` on a gloo group (ranks sharing one GPU) copy the packed message through host memory."""
+    run_ranks(_p2p_routing_worker, 2, timeout=300)
 
 
 def _sharded_worker(rank, world, root, kill):
